@@ -1,6 +1,7 @@
 #!/usr/bin/env python
-"""bench.py — the reference's headline metric on B200: simulated-ms/sec (and msgs/sec) of
-GSFSignature, 131 072 nodes (BASELINE.json), through the C ABI of wittgenstein_b200.
+"""bench.py — the reference's headline metric on H100: simulated-ms/sec (and msgs/sec) of
+GSFSignature, 65 536 nodes (BASELINE.json: the largest power of two whose engine state, ~40 GB, fits the
+H100's 80 GB; 131 072 nodes need ~120 GB), through the C ABI of wittgenstein_b200.
 
 A "step" is one `network.runMs(STEP_MS)` window of one continuing simulation (the reference drives
 its runs the same way: ProgressPerTime.java:79-95 calls runMs in a loop).  W warm-up steps, then
@@ -10,11 +11,15 @@ exactly K timed steps:
            reference's callers read after each runMs (per-node signature count + the 5 node counters)
            and writes/reads the control block — a fresh, identically seeded network, wall clock.
   roofline: dominant kernel of the timed region (per-kernel CUDA-event timing in a third identical
-           pass), algorithmic bytes / its time, against MEASURED_PEAKS.json.
+           pass), algorithmic bytes / its time, against MEASURED_PEAKS.json if present, else the H100 SXM
+           data-sheet HBM3 bandwidth (3.35 TB/s, "peak_source": "fallback").
   cpu_baseline: the CPU oracle (C++ restatement of the reference engine, 1 thread like the reference)
            on a bounded sample of the same workload.
 --impl reference times the reference's CPU path (the oracle port; the Java reference cannot run here:
 no JVM) on the host cores with the same step definition.
+--dump-outputs DIR writes what the device-timed pass computed by its last step (the arrays a caller reads back after
+runMs) as DIR/<name>.npy in float64 / float32, at most 64 MB (see dump_outputs); inputs are seeded, so two builds
+run with the same arguments can be compared output for output.
 """
 import argparse
 import json
@@ -28,6 +33,9 @@ ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 
 AWS_NB, AWS_NL = "AWS_SPEED=GAUSSIAN_TOR=0.33", "AwsRegionNetworkLatency"
+H100_HBM_GBS = 3350.0  # NVIDIA H100 SXM data sheet (700 W card); a roofline denominator, not a measured figure
+DUMP_MAX_BYTES = 64 << 20  # --dump-outputs writes at most this much; larger outputs are sampled on a fixed seed to fit
+DUMP_ROWS = 32             # verifiedSignatures rows dumped (seeded sample), one float32 0/1 per bit, within a quarter of the budget
 
 
 def gsf_params(n):
@@ -38,7 +46,7 @@ def gsf_params(n):
 
 
 class ClockSampler(threading.Thread):
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region (read-only queries)."""
 
     def __init__(self, index):
         super().__init__(daemon=True)
@@ -68,6 +76,66 @@ class ClockSampler(threading.Thread):
         reasons = [n for i, n in enumerate(names) if any(len(r) > 2 + i and r[2 + i].lower().startswith("active") for r in self.rows)]
         return {"sm_mhz": statistics.median(sm) if sm else None, "sm_max_mhz": max(mx) if mx else None, "reasons": reasons,
                 "samples": len(sm)}
+
+
+def dump_outputs(out_dir, arrays, n):
+    """Write `arrays` (name -> (array, axis of the node index), or (array, None) for arrays not indexed by node) as
+    out_dir/<name>.npy: integers as float64 (exact below 2**53), float32 bit rows as float32.  When the per-node arrays of all n
+    nodes do not fit what DUMP_MAX_BYTES leaves after the other arrays, they are written for a fixed, seeded sample of as many
+    nodes as fit; the node ids written are in nodes.npy."""
+    import numpy as np
+
+    def out_dtype(a):
+        return np.float32 if a.dtype == np.float32 else np.float64
+
+    arrays = {name: (np.asarray(a), ax) for name, (a, ax) in arrays.items()}
+    fixed = sum(a.size * np.dtype(out_dtype(a)).itemsize for a, ax in arrays.values() if ax is None)
+    per_node = 8 + sum(a.size // a.shape[ax] * np.dtype(out_dtype(a)).itemsize for a, ax in arrays.values() if ax is not None)
+    k = int(max(1, min(n, (DUMP_MAX_BYTES - fixed) // per_node)))
+    nodes = np.arange(n) if k == n else np.sort(np.random.default_rng(0).choice(n, k, replace=False))
+    out = {"nodes": nodes.astype(np.float64)}
+    for name, (a, ax) in arrays.items():
+        if ax is not None and k < n:
+            a = np.take(a, nodes, axis=ax)
+        out[name] = a.astype(out_dtype(a))
+    os.makedirs(out_dir, exist_ok=True)
+    for name, a in out.items():
+        np.save(os.path.join(out_dir, name + ".npy"), a)
+
+
+def gsf_outputs(p):
+    """What a caller of the GSF timed path reads back after runMs: node counters, per-node and per-level scalars, and a
+    seeded sample of verifiedSignatures rows (bits unpacked)."""
+    import numpy as np
+
+    q = p.local if hasattr(p, "local") else p  # a rank of a node-sharded job dumps its own shard
+    n = int(q.scalars()["card"].shape[0])
+    out = {"counters": (q.network().counters(), 1)}
+    out.update({"scalar_" + k: (v, 0) for k, v in q.scalars().items()})
+    out.update({"level_" + k: (v, 0) for k, v in q.level_scalars().items()})
+    ver = q.verified()
+    row_bytes = ver.shape[1] * 64 * 4
+    rows = np.sort(np.random.default_rng(1).choice(n, max(1, min(DUMP_ROWS, n, DUMP_MAX_BYTES // 4 // row_bytes)), replace=False))
+    ver = ver[rows]
+    bits = np.unpackbits(ver.view(np.uint8), axis=1, bitorder="little").astype(np.float32)
+    out["verified_rows"] = (bits, None)
+    out["verified_row_ids"] = (rows, None)
+    return out, n
+
+
+def casper_outputs(p):
+    """What a caller of the CasperIMD timed path reads back after a slot: node state, heads, counters and the block table."""
+    import numpy as np
+
+    q = p.local if hasattr(p, "local") else p
+    st = q.node_state()
+    out = {"node_" + k: (v, 0) for k, v in st.items() if v.dtype != np.uint64}
+    out.update({"node_" + k + "_lo32": (v & np.uint64(0xFFFFFFFF), 0) for k, v in st.items() if v.dtype == np.uint64})
+    out.update({"node_" + k + "_hi32": (v >> np.uint64(32), 0) for k, v in st.items() if v.dtype == np.uint64})
+    out["heads"] = (q.heads(), 0)
+    out["counters"] = (q.network().counters(), 1)
+    out.update({"block_" + k: (v, None) for k, v in q.blocks().items()})
+    return out, int(out["heads"][0].shape[0])
 
 
 def metric_name(n):
@@ -230,16 +298,6 @@ def cpu_baseline_and_parity(n, args):
     return cpu, parity
 
 
-def ncu_traffic(kernel):
-    """dram__bytes_read.sum + dram__bytes_write.sum per launch of the dominant kernel from the committed ncu capture
-    (profiles/r02_traffic.json, written by scripts/ncu_traffic.py from an `ncu --set full` page); None if absent."""
-    try:
-        t = json.load(open(os.path.join(ROOT, "profiles", "r02_traffic.json")))
-        return t.get(kernel, {}).get("dram_bytes_per_launch")
-    except Exception:
-        return None
-
-
 def feasible_cpu_nodes(n, cap):
     """largest power-of-two node count <= n whose oracle state (peer tables: 4 N^2 bytes) fits in host RAM"""
     import psutil
@@ -327,7 +385,7 @@ def run_casper_reference(args):
 
 def run_casper(args, rank, world, local, dist, barrier, max_over_ranks, sum_over_ranks):
     """--workload casper: SURVEY.md §8d config #4 on the device engine.  N > 1: ONE simulation, node ids sharded over the ranks'
-    GPUs (BASELINE config #4: "node-sharded across 4xB200"; `--mode replicas`: independent seeds instead)."""
+    GPUs (BASELINE config #4: "node-sharded across 4xH100"; `--mode replicas`: independent seeds instead)."""
     import torch
 
     from wittgenstein_b200 import CasperIMD, CasperParemeters
@@ -371,6 +429,8 @@ def run_casper(args, rank, world, local, dist, barrier, max_over_ranks, sum_over
     st1 = net.stats()
     heads_end = p.heads()
     nblocks = len(p.blocks()["height"])
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, *casper_outputs(p))
     del p, net
     # pass 2: end to end with the read-backs a caller makes after every slot (heads + the five node counters)
     p = make()
@@ -437,7 +497,7 @@ def run_casper(args, rank, world, local, dist, barrier, max_over_ranks, sum_over
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    peak = float(peaks.get("hbm_gbs", 6650.0))
+    peak = float(peaks.get("hbm_gbs", H100_HBM_GBS))
     line = {"metric": "simulated-ms/sec, CasperIMD 16,390 nodes", "value": value, "unit": "simulated-ms/s", "n_gpus": world, "steps": K,
             "warmup": W, "ms_per_step": dev_ms / K, "higher_is_better": True, "scaling": "strong" if sharded else "weak", "vs_baseline": None,
             "dtype": "u64 bitmaps / int32", "data": "synthetic",
@@ -477,11 +537,11 @@ def main():
     ap.add_argument("--steps", type=int, default=22)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="b200")
-    ap.add_argument("--nodes", type=int, default=131072)
+    ap.add_argument("--nodes", type=int, default=65536)
     ap.add_argument("--step-ms", type=int, default=0, help="0: ceil(run length / steps)")
     ap.add_argument("--ref-step-ms", type=int, default=20)
-    ap.add_argument("--cpu-nodes", type=int, default=131072)
-    ap.add_argument("--cpu-max-nodes", type=int, default=131072)
+    ap.add_argument("--cpu-nodes", type=int, default=65536)
+    ap.add_argument("--cpu-max-nodes", type=int, default=65536)
     ap.add_argument("--cpu-budget-s", type=float, default=20.0)
     ap.add_argument("--mode", default="auto", choices=["auto", "sharded", "weak", "replicas"],
                     help="N > 1: sharded = ONE simulation of --nodes nodes, node ids sharded over the GPUs (default; strong scaling); "
@@ -489,6 +549,8 @@ def main():
     ap.add_argument("--weak-nodes-per-gpu", type=int, default=32768)
     ap.add_argument("--no-cpu", action="store_true")
     ap.add_argument("--no-profile", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the arrays the timed pass computed in its last step as DIR/<name>.npy")
     args = ap.parse_args()
 
     rank = int(os.environ.get("RANK", "0"))
@@ -571,6 +633,8 @@ def main():
     launches = st1["kernel_launches"] - st0["kernel_launches"]
     card_end = p.scalars()["card"]
     done = not p.continue_if()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, *gsf_outputs(p))
     dev_ms = max_over_ranks(dev_ms)
     ev_all = {k: int(total(v)) for k, v in ev.items()} if sharded else ev
     launches_all = int(total(launches)) if sharded else launches
@@ -644,7 +708,7 @@ def main():
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    peak = float(peaks.get("hbm_gbs", 6650.0))
+    peak = float(peaks.get("hbm_gbs", H100_HBM_GBS))
     roof = None
     if prof:
         ab = algorithmic_bytes(ev)
@@ -654,7 +718,7 @@ def main():
         if kname in ab and kcnt:
             achieved = ab[kname] / (kms / 1000.0) / 1e9
             roof = {"bound": "hbm", "kernel": kname, "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                    "traffic": ncu_traffic(kname), "peak_source": "measured" if peaks else "fallback",
+                    "peak_source": "measured" if peaks else "fallback",
                     "avg_launch_us": 1000.0 * kms / kcnt, "algorithmic_bytes_per_launch": ab[kname] / kcnt,
                     "share_of_step": kms / total_ms,
                     "kernel_ms": {k: round(v[0], 3) for k, v in prof.items()},

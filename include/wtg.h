@@ -1,4 +1,4 @@
-/* wittgenstein_b200 — C ABI of the B200-native simulation engine.
+/* wittgenstein_b200 — C ABI of the H100-native simulation engine.
  *
  * The reference (ConsenSys/wittgenstein, Java) has no FFI of its own: the seam is the Java API
  * `Protocol { network(); copy(); init(); }` (core/Protocol.java:7-22) and the public members of

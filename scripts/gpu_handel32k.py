@@ -1,4 +1,4 @@
-"""BASELINE config #3: Handel 32 768 nodes, 25 % Byzantine (suicide), AwsRegionNetworkLatency, 1 x B200.
+"""BASELINE config #3: Handel 32 768 nodes, 25 % Byzantine (suicide), AwsRegionNetworkLatency, 1 x H100.
 Times the GPU engine to completion and checks the state against the oracle at t = 100 / 300 ms."""
 import json, os, sys, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))

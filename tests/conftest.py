@@ -11,7 +11,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: test needs a CUDA device (run with -m gpu on the B200 box)")
+    config.addinivalue_line("markers", "gpu: test needs a CUDA device (run with -m gpu on an H100)")
 
 
 @pytest.fixture(scope="session")
@@ -22,9 +22,9 @@ def oracle():
 
 
 def pytest_sessionstart(session):
-    # Debugging aid only (never set by the driver): WTG_TEST_EMU=1 routes the C-ABI calls of the `-m gpu`
+    # Debugging aid only: WTG_TEST_EMU=1 routes the C-ABI calls of the `-m gpu`
     # tests to the host-compiled build of the device logic (tests/emu) so that the *test logic* can be
-    # exercised on a machine without a GPU.  Real parity runs happen on the B200 with this unset.
+    # exercised on a machine without a GPU.  Real parity runs happen on an H100 with this unset.
     if os.environ.get("WTG_TEST_EMU") == "1":
         from tests import emu_lib
         from wittgenstein_b200 import _lib

@@ -1,7 +1,7 @@
 // TEST INFRASTRUCTURE.  C++ parity tests through the C++ mirror of the reference classes (include/wtg.hpp, over the C
 // ABI) against the CPU oracle (oracle/*.hpp), written like the reference's own JUnit tests:
 //   PT/PingPongTest.java:8-19, PT/GSFSignatureTest.java:95-124, PT/CasperByzantineTest.java:12-36, PT/HandelTest.java:36-49.
-// Built and run by tests/test_cpp_mirror.py (the run needs a B200: the product library has no CPU fallback).
+// Built and run by tests/test_cpp_mirror.py (the run needs a GPU: the product library has no CPU fallback).
 #include <cstdio>
 #include <cstdlib>
 

@@ -117,10 +117,11 @@ def test_progress_per_time_rounds():
     assert a.average["msg_rcvd"] == sums["msg_rcvd"] // 3 and a.average["done_at"] == sums["done_at"] // 3
 
 
-def test_gsf_131072_prefix_vs_oracle():
-    """The metric configuration itself (BASELINE.json: GSFSignature, 131 072 nodes) against the oracle: bit-exact state
-    after [0, 300] ms with runMs(10) slicing — pooled payload levels up to 18 (8 KiB blocks), 3N-entry buckets.  Needs
-    ~80 GB of host memory for the oracle's peer tables; skipped on smaller hosts."""
+def test_gsf_65536_prefix_vs_oracle():
+    """The metric configuration itself (BASELINE.json: GSFSignature, 65 536 nodes, the largest power of two whose engine
+    state fits an 80 GB H100) against the oracle: bit-exact state after [0, 300] ms with runMs(10) slicing — pooled payload
+    levels up to 17 (4 KiB blocks), 3N-entry buckets.  Needs ~40 GB of host memory for the oracle's peer tables; skipped on
+    smaller hosts."""
     import os
 
     import psutil
@@ -128,9 +129,9 @@ def test_gsf_131072_prefix_vs_oracle():
     from tests import parity
     from tests.oracle_lib import OracleGSF
 
-    n = 131072
-    if psutil.virtual_memory().available < 110 * 2**30:
-        pytest.skip("host memory too small for the oracle at 131072 nodes")
+    n = 65536
+    if psutil.virtual_memory().available < 40 * 2**30:
+        pytest.skip("host memory too small for the oracle at 65536 nodes")
     o = OracleGSF(n, int(0.85 * n), 4, 50, 20, 10, int(0.10 * n), AWS_NB, AWS_NL)
     o.init_fast(min(64, os.cpu_count() or 1))
     p = make(n)

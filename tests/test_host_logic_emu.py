@@ -1,7 +1,7 @@
 """CPU-side regression of the host logic (engine orchestration, init paths, C-ABI argument handling, read-backs) and of the
 state-transition bodies shared between the CUDA kernels and the host debugging build (tests/emu): every protocol, a short
 run, bit-for-bit against the oracle.  TEST INFRASTRUCTURE: the debugging build exports wtgemu_* symbols and is never loaded
-by the product; the parity tests proper (-m gpu) run the CUDA path through the C ABI on a B200."""
+by the product; the parity tests proper (-m gpu) run the CUDA path through the C ABI on an H100."""
 import numpy as np
 import pytest
 

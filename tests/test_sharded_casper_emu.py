@@ -1,4 +1,4 @@
-"""Node-sharded CasperIMD (BASELINE config #4: "CasperIMD ... node-sharded across 4xB200"; DESIGN.md §8), host logic: the
+"""Node-sharded CasperIMD (BASELINE config #4: "CasperIMD ... node-sharded across 4xH100"; DESIGN.md §8), host logic: the
 same state-transition bodies and exchange protocol as the CUDA engine, compiled for the host (tests/emu), G shards driven by
 G threads, checked bit for bit against the oracle — replicated block / attestation tables, sendAll records built on every
 shard, the far-future calendar with ordering keys, and the per-pass "next event" minimum of the fast-forward.

@@ -1,4 +1,4 @@
-"""wittgenstein_b200 — B200-native discrete-event engine behind the Wittgenstein
+"""wittgenstein_b200 — H100-native discrete-event engine behind the Wittgenstein
 Protocol / Network / Node / Message surface (hot path only: see DESIGN.md)."""
 from ._lib import WtgError  # noqa: F401
 from .network import Network  # noqa: F401

@@ -1,8 +1,8 @@
 """ctypes loader for the C-ABI shared library (include/wtg.h).
 
-The library is hand-written CUDA for sm_100a (wittgenstein_b200/csrc).  There is no CPU
+The library is hand-written CUDA for sm_90a (H100; wittgenstein_b200/csrc).  There is no CPU
 fallback: if the shared library is missing or no CUDA device is visible, creating a network
-raises.  Build it with `python -c "import __graft_entry__ as g; g.build()"` or `make -C wittgenstein_b200`.
+raises.  Build it with `python -c "import __graft_entry__ as g; g.build()"`.
 """
 import ctypes as C
 import os

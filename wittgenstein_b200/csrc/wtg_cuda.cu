@@ -1,4 +1,4 @@
-// wittgenstein_b200 — CUDA backend (sm_100a): the kernels of the tick pipeline and the C ABI.
+// wittgenstein_b200 — CUDA backend (sm_90a, H100): the kernels of the tick pipeline and the C ABI.
 //
 // One simulated millisecond = one pass of this kernel sequence over SoA state resident in HBM:
 //   k_begin -> k_cond_mark / k_cond_nodes<scan> / k_cond_score / k_cond_nodes<select> (conditional tasks) ->
@@ -262,7 +262,8 @@ __device__ __forceinline__ void b_node_tasks(const Dev& d, const int VB, const i
   if (c.tma.ready && (threadIdx.x & 31) == 0) bulkWaitAll();
 #endif  // this lane's bulk stores are complete before the kernel ends
 }
-// three blocks per SM = 80 registers: measured best (profiles/README.md, round 2: 64 / 80 / 128 registers -> 258 / 251 / 382 ms)
+// three blocks per SM = at most 80 registers per thread.  GSFSignature 65 536 nodes on an H100 80GB HBM3 (400 W), simulated-ms/s:
+// 80 registers 4 643-4 667 over five runs, 64 (spills ~1 KB) 4 756 and 4 643 in two, 128 4 559 in one: no budget is clearly faster
 __global__ void __launch_bounds__(256, 3) k_node_tasks(Dev d) { b_node_tasks(d, blockIdx.x, gridDim.x); }
 // CasperIMD, after the parallel handler pass (one warp; both are rare): nodes that hit a fork-choice tie run in processing
 // order with their exact draw index (randomOnTies), and several blocks created in one millisecond get their ids in
@@ -660,7 +661,7 @@ __device__ __forceinline__ void b_free(const Dev& d, const int VB, const int VG)
 }
 __global__ void k_free(Dev d) { b_free(d, blockIdx.x, gridDim.x); }
 
-#if defined(WTG_PERSISTENT_WINDOW)  // experiment kept for reference (profiles/README.md, round 2): slower than the graph at the metric size
+#if defined(WTG_PERSISTENT_WINDOW)  // experiment kept for reference (DESIGN.md §6): slower than the per-tick graph on an H100 at 16 384 and 65 536 nodes
 // ---- one cooperative kernel per runMs window ------------------------------------------------------------------
 // The pipeline's kernels are tiny at most ticks (a launch boundary costs more than the work), so a whole window runs as
 // ONE cooperative launch: every stage is a grid-stride loop over the virtual blocks of the stage's stand-alone launch
@@ -801,7 +802,7 @@ class CudaBackend : public Backend {
   cudaStream_t st = nullptr;
   int devId = 0;  // every entry point binds it: callers may drive different networks from different host threads
   void bind() const { cudaSetDevice(devId); }
-  int sms = 148;
+  int sms = 132;
   int smemOptin = 0;
   cudaGraphExec_t tickGraph = nullptr;
   const void* graphFor = nullptr;

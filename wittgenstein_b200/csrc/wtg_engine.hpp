@@ -530,7 +530,7 @@ class Engine {
     const int N = p.nodeCount;
     if (p.nodesDown >= N || p.nodesDown < 0 || p.threshold > N || (p.nodesDown + p.threshold > N))  // :69-74
       throw std::invalid_argument("nodeCount=" + std::to_string(N) + ", threshold=" + std::to_string(p.threshold));
-    if (N < 2 || (N & (N - 1)) != 0) throw std::invalid_argument("the B200 engine needs a power-of-two nodeCount >= 2 for GSFSignature");
+    if (N < 2 || (N & (N - 1)) != 0) throw std::invalid_argument("the device engine needs a power-of-two nodeCount >= 2 for GSFSignature");
     if (p.acceleratedCallsCount > MAX_ACC || p.acceleratedCallsCount < 0) throw std::invalid_argument("acceleratedCallsCount must be in [0,16]");
     if (p.periodDurationMs <= 0 || p.pairingTime < 0) throw std::invalid_argument("period/pairing");
     checkLatencyBuilder();
@@ -707,7 +707,7 @@ class Engine {
     requireNotInited();
     if (sfConstructed) throw std::logic_error("already constructed");
     const int N = p.nodeCount;
-    if (N < 2 || (N & (N - 1)) != 0) throw std::invalid_argument("the B200 engine needs a power-of-two nodeCount >= 2 for SanFerminSignature");
+    if (N < 2 || (N & (N - 1)) != 0) throw std::invalid_argument("the device engine needs a power-of-two nodeCount >= 2 for SanFerminSignature");
     if (p.candidateCount < 1 || p.candidateCount + 1 > SHUFFLE_MAX) throw std::invalid_argument("candidateCount must be in [1, 63]");
     if (p.pairingTime <= 0 || p.replyTimeout <= 0) throw std::invalid_argument("pairingTime / replyTimeout must be positive");
     checkLatencyBuilder();
@@ -1026,7 +1026,7 @@ class Engine {
     requireNotInited();
     requireUnsharded("this protocol");
     const int N = p.nodeCount;
-    if (N < 2 || (N & (N - 1)) != 0) throw std::invalid_argument("the B200 engine needs a power-of-two nodeCount >= 2 for SanFerminCappos");
+    if (N < 2 || (N & (N - 1)) != 0) throw std::invalid_argument("the device engine needs a power-of-two nodeCount >= 2 for SanFerminCappos");
     if (p.candidateCount < 1 || p.candidateCount + 1 > SHUFFLE_MAX) throw std::invalid_argument("candidateCount must be in [1, 63]");
     if (p.pairingTime <= 0 || p.timeout <= 0) throw std::invalid_argument("pairingTime / timeout must be positive");
     checkLatencyBuilder();

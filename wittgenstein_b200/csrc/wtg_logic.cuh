@@ -1196,7 +1196,7 @@ __device__ __forceinline__ void gsfCycleWarp(const Dev& d, CoopWarp& c, int n, i
   }
   unsigned pm = __ballot_sync(FULLM, pooled);
   unsigned long long words = 0;
-#if defined(WTG_TMA_SNAPSHOT)  // experiment kept for reference (profiles/README.md, round 2): slower than the lane-strided copy
+#if defined(WTG_TMA_SNAPSHOT)  // experiment kept for reference (DESIGN.md §6): slower than the lane-strided copy on an H100
   if (pm && c.tma.buf != nullptr) {
     // The snapshots of all sending levels are nested sub-ranges of ONE range of the row: the block of the highest sending
     // level (every level block contains n).  It is read once, by bulk asynchronous copies into this warp's shared-memory

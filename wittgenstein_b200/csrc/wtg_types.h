@@ -1,4 +1,4 @@
-// wittgenstein_b200 — B200-native discrete-event engine behind the reference's
+// wittgenstein_b200 — H100-native discrete-event engine behind the reference's
 // Protocol / Network / Node / Message surface.  Shared POD types (host + device).
 //
 // Data layout in HBM (see DESIGN.md §3):

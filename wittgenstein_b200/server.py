@@ -7,7 +7,7 @@ simple class name in the property `type`), core/External.java.
 
 `Server` mirrors `Server.java` method by method on top of the Python mirror of the protocol classes (one C-ABI call per
 method); `create_app()` exposes it with the same routes, verbs and JSON field names as `WServer.java`, so that the
-reference's web UI (wserver/src/main/resources/static) and HTTP clients can drive the B200 engine.  Differences, all
+reference's web UI (wserver/src/main/resources/static) and HTTP clients can drive the device engine.  Differences, all
 reported as HTTP errors instead of being guessed:
   * `POST /w/network/nodes/{id}/external` (Server.setExternal): a per-delivery HTTP callback cannot run inside a device
     handler -> 501 (SURVEY.md §8b: host-defined `Message.action` bodies are not part of the accelerated ABI);
