@@ -8,7 +8,6 @@
 // All sizes are read from the device control block, so a whole runMs window is enqueued without
 // a host round trip.  See DESIGN.md §4 for why this reproduces the reference's sequential order.
 #include <cuda_runtime.h>
-#include <cooperative_groups.h>
 #include <unistd.h>
 
 #include <cstdio>
@@ -19,7 +18,6 @@
 
 #include "wtg_engine.hpp"
 
-namespace cg = cooperative_groups;
 namespace wtg {
 
 #define CUDA_OK(x)                                                                                       \
@@ -28,17 +26,11 @@ namespace wtg {
     if (e_ != cudaSuccess) throw std::runtime_error(std::string("CUDA: ") + cudaGetErrorString(e_) + " at " #x); \
   } while (0)
 
-#if defined(WTG_TMA_SNAPSHOT)
-constexpr int NODE_TMA_SMEM = 8 * TMA_TILES * TMA_TILE_BYTES;
-#else
-constexpr int NODE_TMA_SMEM = 0;
-#endif
-//  // dynamic shared memory of k_node_tasks (GSF): bulk-copy tiles
 constexpr int SCAN_THREADS = 256;
 constexpr int SCAN_ITEMS = 4;
 constexpr int SCAN_TILE = SCAN_THREADS * SCAN_ITEMS;
 
-__device__ __forceinline__ void b_begin(const Dev& d, int mode, const int VB, const int VG) {  // one warp
+__global__ void k_begin(Dev d, int mode) {  // one warp
   if (threadIdx.x >= 32) return;
   if (d.ffwd && mode == 1) {
     CoopWarp c;
@@ -50,19 +42,18 @@ __device__ __forceinline__ void b_begin(const Dev& d, int mode, const int VB, co
     tickBegin(d, mode);
   }
 }
-__global__ void k_begin(Dev d, int mode) { b_begin(d, mode, blockIdx.x, gridDim.x); }
-__device__ __forceinline__ void b_end(const Dev& d, int mode, const int VB, const int VG) {
+__global__ void k_end(Dev d, int mode) {
   if (threadIdx.x == 0) tickEnd(d, mode);
 }
-__global__ void k_end(Dev d, int mode) { b_end(d, mode, blockIdx.x, gridDim.x); }
 
 // ---- conditional tasks (checkSigs): scan -> score -> select ---------------------------------------
 // append node n to a striped list (stripe = global warp index & 63; a stripe receives at most listStripeCap nodes)
-__device__ __forceinline__ void listAppend(const Dev& d, bool active, int n, int* cnt, int* list, int VB) {
+__device__ __forceinline__ void listAppend(const Dev& d, bool active, int n, int* cnt, int* list) {
   unsigned m = __ballot_sync(0xffffffffu, active);
   if (!m) return;
   int lane = threadIdx.x & 31;
-  int gw = (VB * blockDim.x + threadIdx.x) >> 5;
+  const int blk = blockIdx.x;
+  int gw = (blk * blockDim.x + threadIdx.x) >> 5;
   int stripe = gw & (ARENA_STRIPES - 1);
   int base = 0;
   if (lane == 0) base = atomicAdd(&cnt[stripe], __popc(m));
@@ -70,11 +61,12 @@ __device__ __forceinline__ void listAppend(const Dev& d, bool active, int n, int
   if (active) list[(size_t)stripe * d.listStripeCap + base + __popc(m & ((1u << lane) - 1u))] = n;
 }
 // same, with a 64-bit payload per entry
-__device__ __forceinline__ void listAppendW(const Dev& d, bool active, int n, u64 word, int* cnt, int* list, u64* words, int VB) {
+__device__ __forceinline__ void listAppendW(const Dev& d, bool active, int n, u64 word, int* cnt, int* list, u64* words) {
   unsigned m = __ballot_sync(0xffffffffu, active);
   if (!m) return;
   int lane = threadIdx.x & 31;
-  int gw = (VB * blockDim.x + threadIdx.x) >> 5;
+  const int blk = blockIdx.x;
+  int gw = (blk * blockDim.x + threadIdx.x) >> 5;
   int stripe = gw & (ARENA_STRIPES - 1);
   int base = 0;
   if (lane == 0) base = atomicAdd(&cnt[stripe], __popc(m));
@@ -86,25 +78,26 @@ __device__ __forceinline__ void listAppendW(const Dev& d, bool active, int n, u6
   }
 }
 // conditional-task bookkeeping, one thread per node -> list of due nodes
-__device__ __forceinline__ void b_cond_mark(const Dev& d, const int VB, const int VG) {
+__global__ void __launch_bounds__(256) k_cond_mark(Dev d) {
   if (d.ctl->error) return;
-  int n = d.n0 + VB * blockDim.x + threadIdx.x;
+  const int blk = blockIdx.x;
+  int n = d.n0 + blk * blockDim.x + threadIdx.x;
   bool due = false;
   if (n < d.n0 + d.nLoc) due = d.proto == PROTO_HANDEL ? hCondMark(d, n) : gsfCondMark(d, n);
-  listAppend(d, due, n, d.ctl->dueCnt, d.dueList, VB);
+  listAppend(d, due, n, d.ctl->dueCnt, d.dueList);
 }
-__global__ void __launch_bounds__(256) k_cond_mark(Dev d) { b_cond_mark(d, blockIdx.x, gridDim.x); }
 // one warp per due node, blocks assigned to list stripes
 template <int PHASE>
-__device__ __forceinline__ void b_cond_nodes(const Dev& d, const int VB, const int VG) {
+__global__ void __launch_bounds__(256) k_cond_nodes(Dev d) {
   extern __shared__ uint32_t keepAll[];
   __shared__ HScratch scratch[8];
   if (d.ctl->error) return;
-  const int stripe = VB & (ARENA_STRIPES - 1);
+  const int blk = blockIdx.x, nBlk = gridDim.x;
+  const int stripe = blk & (ARENA_STRIPES - 1);
   const int cnt = d.ctl->dueCnt[stripe];
   const int warp = threadIdx.x >> 5;
-  const int sub = (VB >> 6) * 8 + warp;
-  const int nsub = (VG >> 6) * 8;
+  const int sub = (blk >> 6) * 8 + warp;
+  const int nsub = (nBlk >> 6) * 8;
   const int* list = d.dueList + (size_t)stripe * d.listStripeCap;
   CoopWarp c;
   for (int t = sub; t < cnt; t += nsub) {
@@ -122,18 +115,17 @@ __device__ __forceinline__ void b_cond_nodes(const Dev& d, const int VB, const i
     }
   }
 }
-template <int PHASE>
-__global__ void __launch_bounds__(256) k_cond_nodes(Dev d) { b_cond_nodes<PHASE>(d, blockIdx.x, gridDim.x); }
 // blocks are assigned to arena stripes (blockIdx & 63), so an item is found without walking the 64 counters
-__device__ __forceinline__ void b_cond_score(const Dev& d, const int VB, const int VG) {
+__global__ void __launch_bounds__(256) k_cond_score(Dev d) {
   if (d.ctl->error) return;
+  const int blk = blockIdx.x, nBlk = gridDim.x;
   const int per = d.workCap / ARENA_STRIPES;
-  const int stripe = VB & (ARENA_STRIPES - 1);
+  const int stripe = blk & (ARENA_STRIPES - 1);
   int cnt = d.ctl->workCnt[stripe];
   if (cnt > per) cnt = per;
   const int warpsPerBlock = blockDim.x >> 5;
-  const int sub = (VB >> 6) * warpsPerBlock + (threadIdx.x >> 5);
-  const int nsub = (VG >> 6) * warpsPerBlock;
+  const int sub = (blk >> 6) * warpsPerBlock + (threadIdx.x >> 5);
+  const int nsub = (nBlk >> 6) * warpsPerBlock;
   CoopWarp c;
   const uint32_t* wl = d.workList + (size_t)stripe * per;
   for (int t = sub; t < cnt; t += nsub) {
@@ -144,58 +136,58 @@ __device__ __forceinline__ void b_cond_score(const Dev& d, const int VB, const i
       gsfScoreItem(d, c, it);
   }
 }
-__global__ void __launch_bounds__(256) k_cond_score(Dev d) { b_cond_score(d, blockIdx.x, gridDim.x); }
 // ---- Handel conditional pass (checkSigs): scan -> score -> select -> draw scan -> pick ---------------------
 // does any nextInt(k) of this pass hit java.util.Random's rejection loop?  (probability ~ k / 2^31 per draw)
-__device__ __forceinline__ void b_hpick_check(const Dev& d, const int VB, const int VG) {
+__global__ void k_hpick_check(Dev d) {
   if (d.ctl->error) return;
-  for (int n = d.n0 + VB * blockDim.x + threadIdx.x; n < d.n0 + d.nLoc; n += VG * blockDim.x)
+  const int blk = blockIdx.x, nBlk = gridDim.x;
+  for (int n = d.n0 + blk * blockDim.x + threadIdx.x; n < d.n0 + d.nLoc; n += nBlk * blockDim.x)
     if (d.hCandK[n] > 0 && hCondPick(d, n, (u64)d.hDrawBase[n], false) > d.condDraws[n]) d.ctl->hReject = 1;
 }
-__global__ void k_hpick_check(Dev d) { b_hpick_check(d, blockIdx.x, gridDim.x); }
-__device__ __forceinline__ void b_hpick_apply(const Dev& d, const int VB, const int VG) {
+__global__ void k_hpick_apply(Dev d) {
   if (d.ctl->error) return;
+  const int blk = blockIdx.x, nBlk = gridDim.x;
   if (!d.ctl->hReject) {
-    for (int n = d.n0 + VB * blockDim.x + threadIdx.x; n < d.n0 + d.nLoc; n += VG * blockDim.x) hCondPick(d, n, (u64)d.hDrawBase[n], true);
-  } else if (VB == 0 && threadIdx.x == 0) {  // a rejection shifts every later draw: redo the picks in node order
+    for (int n = d.n0 + blk * blockDim.x + threadIdx.x; n < d.n0 + d.nLoc; n += nBlk * blockDim.x) hCondPick(d, n, (u64)d.hDrawBase[n], true);
+  } else if (blk == 0 && threadIdx.x == 0) {  // a rejection shifts every later draw: redo the picks in node order
     u64 idx = 0;
     for (int n = d.n0; n < d.n0 + d.nLoc; ++n) idx += (u64)hCondPick(d, n, idx, true);
   }
 }
-__global__ void k_hpick_apply(Dev d) { b_hpick_apply(d, blockIdx.x, gridDim.x); }
 
 // ---- dispatch -----------------------------------------------------------------------------
-__device__ __forceinline__ void b_dispatch_count(const Dev& d, const int VB, const int VG) {
+__global__ void k_dispatch_count(Dev d) {
   if (d.ctl->error) return;
+  const int blk = blockIdx.x, nBlk = gridDim.x;
   int nEv = d.ctl->nEv;
   if (d.allCap > 0) {  // sendAll protocols: a warp per bucket entry
     CoopWarp c;
-    int gw = (VB * blockDim.x + threadIdx.x) >> 5, nw = (VG * blockDim.x) >> 5;
+    int gw = (blk * blockDim.x + threadIdx.x) >> 5, nw = (nBlk * blockDim.x) >> 5;
     for (int i = gw; i < nEv; i += nw) dispatchCountCoop(d, c, i);
     return;
   }
-  for (int i = VB * blockDim.x + threadIdx.x; i < nEv; i += VG * blockDim.x) dispatchCount(d, i);
+  for (int i = blk * blockDim.x + threadIdx.x; i < nEv; i += nBlk * blockDim.x) dispatchCount(d, i);
 }
-__global__ void k_dispatch_count(Dev d) { b_dispatch_count(d, blockIdx.x, gridDim.x); }
-__device__ __forceinline__ void b_dispatch_scatter(const Dev& d, const int VB, const int VG) {
+__global__ void k_dispatch_scatter(Dev d) {
   if (d.ctl->error) return;
+  const int blk = blockIdx.x, nBlk = gridDim.x;
   int nEv = d.ctl->nEv;
   if (d.allCap > 0) {
     CoopWarp c;
-    int gw = (VB * blockDim.x + threadIdx.x) >> 5, nw = (VG * blockDim.x) >> 5;
+    int gw = (blk * blockDim.x + threadIdx.x) >> 5, nw = (nBlk * blockDim.x) >> 5;
     for (int i = gw; i < nEv; i += nw) dispatchScatterCoop(d, c, i);
     return;
   }
-  for (int i = VB * blockDim.x + threadIdx.x; i < nEv; i += VG * blockDim.x) dispatchScatter(d, i);
+  for (int i = blk * blockDim.x + threadIdx.x; i < nEv; i += nBlk * blockDim.x) dispatchScatter(d, i);
 }
-__global__ void k_dispatch_scatter(Dev d) { b_dispatch_scatter(d, blockIdx.x, gridDim.x); }
 
 // ---- handlers: warp per node ----------------------------------------------------------------
 // pass 1: one thread per node.  GSF / PingPong: message deliveries (they commute with the node's tasks, see
 // nodeProcess); SanFermin: everything (all handlers are scalar).  Leaves nodeTasks[n] = 1 when a warp is needed.
-__device__ __forceinline__ void b_node_msgs(const Dev& d, const int VB, const int VG) {
+__global__ void __launch_bounds__(256) k_node_msgs(Dev d) {
   if (d.ctl->error) return;
-  int n = d.n0 + VB * blockDim.x + threadIdx.x;
+  const int blk = blockIdx.x;
+  int n = d.n0 + blk * blockDim.x + threadIdx.x;
   int flag = 0;
   u64 word = ~0ULL;
   if (n < d.n0 + d.nLoc && d.inboxFill[n] > 0) {
@@ -225,31 +217,23 @@ __device__ __forceinline__ void b_node_msgs(const Dev& d, const int VB, const in
     } else
       flag = 1;
   }
-  listAppendW(d, flag != 0, n, word, d.ctl->taskCnt, d.taskList, d.taskWord, VB);
+  listAppendW(d, flag != 0, n, word, d.ctl->taskCnt, d.taskList, d.taskWord);
 }
-__global__ void __launch_bounds__(256) k_node_msgs(Dev d) { b_node_msgs(d, blockIdx.x, gridDim.x); }
 // pass 2: one warp per node that has tasks (updateVerifiedSignatures / doCycle / ...), or, for protocols whose
 // events do not commute (Handel), all of the node's events in reference order; blocks assigned to list stripes.
-__device__ __forceinline__ void b_node_tasks(const Dev& d, const int VB, const int VG) {
-  // bulk-copy tiles and their mbarriers, one set per warp (wtg_tma.cuh): payload snapshots of doCycle
-  CoopWarp c;
-#if defined(WTG_TMA_SNAPSHOT)
-  extern __shared__ __align__(128) unsigned long long tmaTiles[];  // [8 warps][TMA_TILES * TMA_TILE_BYTES / 8] (dynamic: NODE_TMA_SMEM)
-  __shared__ __align__(8) unsigned long long tmaBars[8][TMA_TILES];
-  if (d.proto == PROTO_GSF) {  // the mbarriers are initialised by the first snapshot of the warp (most launches have none)
-    const int warp = threadIdx.x >> 5;
-    c.tma.buf = tmaTiles + (size_t)warp * (TMA_TILES * TMA_TILE_BYTES / 8);
-    c.tma.bar = &tmaBars[warp][0];
-  }
-#endif
+// Three blocks per SM = at most 80 registers per thread.  GSFSignature 65 536 nodes on an H100 80GB HBM3 (400 W), simulated-ms/s:
+// 80 registers 4 643-4 667 over five runs, 64 (spills ~1 KB) 4 756 and 4 643 in two, 128 4 559 in one: no budget is clearly faster
+__global__ void __launch_bounds__(256, 3) k_node_tasks(Dev d) {
   if (d.ctl->error) return;
+  const int blk = blockIdx.x, nBlk = gridDim.x;
   const bool split = d.proto == PROTO_GSF || d.proto == PROTO_PINGPONG;
-  const int stripe = VB & (ARENA_STRIPES - 1);
+  const int stripe = blk & (ARENA_STRIPES - 1);
   const int cnt = d.ctl->taskCnt[stripe];
-  const int sub = (VB >> 6) * 8 + (threadIdx.x >> 5);
-  const int nsub = (VG >> 6) * 8;
+  const int sub = (blk >> 6) * 8 + (threadIdx.x >> 5);
+  const int nsub = (nBlk >> 6) * 8;
   const int* list = d.taskList + (size_t)stripe * d.listStripeCap;
   const u64* words = d.taskWord + (size_t)stripe * d.listStripeCap;
+  CoopWarp c;
   for (int t = sub; t < cnt; t += nsub) {
     const int n = list[t];
     const u64 w = words[t];
@@ -258,23 +242,17 @@ __device__ __forceinline__ void b_node_tasks(const Dev& d, const int VB, const i
     else
       nodeProcess(d, c, n, split ? 2 : 0);
   }
-#if defined(WTG_TMA_SNAPSHOT)
-  if (c.tma.ready && (threadIdx.x & 31) == 0) bulkWaitAll();
-#endif  // this lane's bulk stores are complete before the kernel ends
 }
-// three blocks per SM = at most 80 registers per thread.  GSFSignature 65 536 nodes on an H100 80GB HBM3 (400 W), simulated-ms/s:
-// 80 registers 4 643-4 667 over five runs, 64 (spills ~1 KB) 4 756 and 4 643 in two, 128 4 559 in one: no budget is clearly faster
-__global__ void __launch_bounds__(256, 3) k_node_tasks(Dev d) { b_node_tasks(d, blockIdx.x, gridDim.x); }
 // CasperIMD, after the parallel handler pass (one warp; both are rare): nodes that hit a fork-choice tie run in processing
 // order with their exact draw index (randomOnTies), and several blocks created in one millisecond get their ids in
 // processing order
-__device__ __forceinline__ void b_casper_fixups(const Dev& d, const int VB, const int VG) {
-  if (d.ctl->error || VB != 0 || threadIdx.x >= 32) return;
+__global__ void k_casper_fixups(Dev d) {
+  const int blk = blockIdx.x;
+  if (d.ctl->error || blk != 0 || threadIdx.x >= 32) return;
   CoopWarp c;
   if (d.cRandomTies && d.ctl->tieCnt > 0) casperResolveTies(d, c);
   if (d.G == 1 && d.cg->createdThisTick > 1) casperRenumber(d, c);
 }
-__global__ void k_casper_fixups(Dev d) { b_casper_fixups(d, blockIdx.x, gridDim.x); }
 // ---- pair scans ---------------------------------------------------------------------------
 __device__ __forceinline__ Pair pairAdd(Pair x, Pair y) {
   Pair r;
@@ -326,11 +304,12 @@ __device__ __forceinline__ Pair blockExclusive(Pair v, Pair& total) {
   return r;
 }
 
-__device__ __forceinline__ void b_scan_partial(const Dev& d, int which, const int VB, const int VG) {
+__global__ void __launch_bounds__(SCAN_THREADS) k_scan_partial(Dev d, int which) {
   if (d.ctl->error) return;
+  const int blk = blockIdx.x, nBlk = gridDim.x;
   int M = scanCount(d, which);
   int nTiles = (M + SCAN_TILE - 1) / SCAN_TILE;
-  for (int tile = VB; tile < nTiles; tile += VG) {
+  for (int tile = blk; tile < nTiles; tile += nBlk) {
     int j0 = tile * SCAN_TILE + threadIdx.x * SCAN_ITEMS;
     Pair s;
     s.a = 0;
@@ -347,20 +326,20 @@ __device__ __forceinline__ void b_scan_partial(const Dev& d, int which, const in
     __syncthreads();
   }
 }
-__global__ void __launch_bounds__(SCAN_THREADS) k_scan_partial(Dev d, int which) { b_scan_partial(d, which, blockIdx.x, gridDim.x); }
 // second (last) scan kernel: every block first sums the partials of the tiles before its own (a few hundred
 // pairs at most), then scans its tile; the block of the last tile also publishes the totals.
-__device__ __forceinline__ void b_scan_final(const Dev& d, int which, const int VB, const int VG) {
+__global__ void __launch_bounds__(SCAN_THREADS) k_scan_final(Dev d, int which) {
   if (d.ctl->error) return;
+  const int blk = blockIdx.x, nBlk = gridDim.x;
   int M = scanCount(d, which);
   int nTiles = (M + SCAN_TILE - 1) / SCAN_TILE;
-  if (nTiles == 0 && VB == 0 && threadIdx.x == 0) {
+  if (nTiles == 0 && blk == 0 && threadIdx.x == 0) {
     Pair z;
     z.a = 0;
     z.b = 0;
     scanTotals(d, which, z);
   }
-  for (int tile = VB; tile < nTiles; tile += VG) {
+  for (int tile = blk; tile < nTiles; tile += nBlk) {
     Pair pre;
     pre.a = 0;
     pre.b = 0;
@@ -397,64 +376,61 @@ __device__ __forceinline__ void b_scan_final(const Dev& d, int which, const int 
     __syncthreads();
   }
 }
-__global__ void __launch_bounds__(SCAN_THREADS) k_scan_final(Dev d, int which) { b_scan_final(d, which, blockIdx.x, gridDim.x); }
 
 // ---- shuffled multi-sends: optimistic draw indices, checked; re-derived serially when a rejection shifted them ----
-__device__ __forceinline__ void b_shuffle_check(const Dev& d, const int VB, const int VG) {
+__global__ void k_shuffle_check(Dev d) {
   if (d.ctl->error) return;
+  const int blk = blockIdx.x, nBlk = gridDim.x;
   const int per = d.descCap / ARENA_STRIPES;
-  const int stripe = VB & (ARENA_STRIPES - 1);
+  const int stripe = blk & (ARENA_STRIPES - 1);
   int cnt = d.ctl->descCnt[stripe];
   if (cnt > per) cnt = per;
-  const int sub = (VB >> 6) * blockDim.x + threadIdx.x;
-  const int nsub = (VG >> 6) * blockDim.x;
+  const int sub = (blk >> 6) * blockDim.x + threadIdx.x;
+  const int nsub = (nBlk >> 6) * blockDim.x;
   for (int j = sub; j < cnt; j += nsub) shuffleCheck(d, stripe * per + j);
 }
-__global__ void k_shuffle_check(Dev d) { b_shuffle_check(d, blockIdx.x, gridDim.x); }
-__device__ __forceinline__ void b_shuffle_serial(const Dev& d, const int VB, const int VG) {
+__global__ void k_shuffle_serial(Dev d) {
   if (d.ctl->error) return;
   shuffleSerial(d);
 }
-__global__ void k_shuffle_serial(Dev d) { b_shuffle_serial(d, blockIdx.x, gridDim.x); }
 
 // ---- node-sharded runs: the two exchanges of a pass (wtg_shard.cuh) --------------------------------------------
 // exchange 1, publication: every item of this shard (key, prefix of slots / draws) into every shard's copy of this shard's
 // list — peer stores over NVLink; a shard in error still publishes its header (which carries the error) so that the
 // others stop at once
-__device__ __forceinline__ void b_x1_publish(const Dev& d, const int VB, const int VG) {
+__global__ void __launch_bounds__(256) k_x1_publish(Dev d) {
+  const int blk = blockIdx.x, nBlk = gridDim.x;
   const int n = d.ctl->error ? -1 : d.ctl->nItems;
-  for (int i = VB * blockDim.x + threadIdx.x; i <= n; i += VG * blockDim.x) xPublishItem(d, i);
-  if (VB == 0 && threadIdx.x == 0) xPublishHeader(d);
+  for (int i = blk * blockDim.x + threadIdx.x; i <= n; i += nBlk * blockDim.x) xPublishItem(d, i);
+  if (blk == 0 && threadIdx.x == 0) xPublishHeader(d);
 }
-__global__ void __launch_bounds__(256) k_x1_publish(Dev d) { b_x1_publish(d, blockIdx.x, gridDim.x); }
 // signal the end of this shard's publication of `phase` to every shard, then wait for all of theirs (one block:
 // spinning must not occupy the machine — shards may share a GPU in the tests)
-__device__ __forceinline__ void b_x_sync(const Dev& d, int phase, const int VB, const int VG) {
+__global__ void k_x_sync(Dev d, int phase) {
   if (threadIdx.x == 0) xSignal(d, phase);  // stream order: the publishing kernel has completed
   __syncthreads();
   if (threadIdx.x < d.G && threadIdx.x != d.rank) xWaitOne(d, phase, threadIdx.x);
 }
-__global__ void k_x_sync(Dev d, int phase) { b_x_sync(d, phase, blockIdx.x, gridDim.x); }
 // exchange 1, evaluation: global totals, and for every local item that created something the creation indices / draws
 // of the other shards that come first
-__device__ __forceinline__ void b_x1_offsets(const Dev& d, const int VB, const int VG) {
+__global__ void __launch_bounds__(256) k_x1_offsets(Dev d) {
   if (d.ctl->error) return;
+  const int blk = blockIdx.x, nBlk = gridDim.x;
   const int n = d.ctl->nItems;
-  for (int i = VB * blockDim.x + threadIdx.x; i < n; i += VG * blockDim.x) xOffsets(d, i);
+  for (int i = blk * blockDim.x + threadIdx.x; i < n; i += nBlk * blockDim.x) xOffsets(d, i);
 }
-__global__ void __launch_bounds__(256) k_x1_offsets(Dev d) { b_x1_offsets(d, blockIdx.x, gridDim.x); }
-__device__ __forceinline__ void b_x1_totals(const Dev& d, const int VB, const int VG) {
+__global__ void k_x1_totals(Dev d) {
   if (d.ctl->error) return;
   xTotals(d);
 }
-__global__ void k_x1_totals(Dev d) { b_x1_totals(d, blockIdx.x, gridDim.x); }
 // exchange 2, after the wait: pooled payloads that arrived in the staging area move into pool slabs (warp per envelope)
-__device__ __forceinline__ void b_x2_ingest(const Dev& d, const int VB, const int VG) {
+__global__ void __launch_bounds__(256) k_x2_ingest(Dev d) {
   if (d.ctl->error) return;
+  const int blk = blockIdx.x, nBlk = gridDim.x;
   const int G = d.ctl->totalSlots;
   CoopWarp c;
   const int lane = threadIdx.x & 31;
-  const int gw = (VB * blockDim.x + threadIdx.x) >> 5, nw = (VG * blockDim.x) >> 5;
+  const int gw = (blk * blockDim.x + threadIdx.x) >> 5, nw = (nBlk * blockDim.x) >> 5;
   for (int g0 = gw * 32; g0 < G; g0 += nw * 32) {
     int g = g0 + lane;
     unsigned m = __ballot_sync(0xffffffffu, g < G && xNeedsIngest(d, g));
@@ -465,57 +441,56 @@ __device__ __forceinline__ void b_x2_ingest(const Dev& d, const int VB, const in
     }
   }
 }
-__global__ void __launch_bounds__(256) k_x2_ingest(Dev d) { b_x2_ingest(d, blockIdx.x, gridDim.x); }
 
 // ---- emit ------------------------------------------------------------------------------------
-__device__ __forceinline__ void b_emit(const Dev& d, const int VB, const int VG) {
+__global__ void k_emit(Dev d) {
   if (d.ctl->error) return;
+  const int blk = blockIdx.x, nBlk = gridDim.x;
   // conditional-task inserts (one per node) ...
-  for (int i = VB * blockDim.x + threadIdx.x; i < d.nLoc; i += VG * blockDim.x) emitCond(d, d.n0 + i);
+  for (int i = blk * blockDim.x + threadIdx.x; i < d.nLoc; i += nBlk * blockDim.x) emitCond(d, d.n0 + i);
   // ... then the handlers' descriptors, blocks assigned to arena stripes
   const int per = d.descCap / ARENA_STRIPES;
-  const int stripe = VB & (ARENA_STRIPES - 1);
+  const int stripe = blk & (ARENA_STRIPES - 1);
   int cnt = d.ctl->descCnt[stripe];
   if (cnt > per) cnt = per;
-  const int sub = (VB >> 6) * blockDim.x + threadIdx.x;
-  const int nsub = (VG >> 6) * blockDim.x;
+  const int sub = (blk >> 6) * blockDim.x + threadIdx.x;
+  const int nsub = (nBlk >> 6) * blockDim.x;
   for (int j = sub; j < cnt; j += nsub) emitDesc(d, stripe * per + j);
 }
-__global__ void k_emit(Dev d) { b_emit(d, blockIdx.x, gridDim.x); }
 
 // sendAll descriptors: one warp each (arrival per destination, stable counting sort by arrival)
-__device__ __forceinline__ void b_emit_all(const Dev& d, const int VB, const int VG) {
+__global__ void __launch_bounds__(128) k_emit_all(Dev d) {
   __shared__ int hist[4][ALL_HIST];
   if (d.ctl->error) return;
+  const int blk = blockIdx.x, nBlk = gridDim.x;
   int cnt = d.ctl->allCnt;
   if (cnt > d.allCap) cnt = d.allCap;
   const int warp = threadIdx.x >> 5;
   if (warp >= 4) return;  // four histograms per block
-  const int gw = VB * 4 + warp, nw = VG * 4;
+  const int gw = blk * 4 + warp, nw = nBlk * 4;
   CoopWarp c;
   for (int j = gw; j < cnt; j += nw) emitAll(d, c, d.allList[j], d.allTmp + (size_t)gw * d.N, hist[warp]);
 }
-__global__ void __launch_bounds__(128) k_emit_all(Dev d) { b_emit_all(d, blockIdx.x, gridDim.x); }
 // node-sharded sendAll (CasperIMD): the descriptors are published to every shard before the envelope exchange ...
-__device__ __forceinline__ void b_x_all_publish(const Dev& d, const int VB, const int VG) {
+__global__ void __launch_bounds__(128) k_x_all_publish(Dev d) {
+  const int blk = blockIdx.x, nBlk = gridDim.x;
   int cnt = d.ctl->error ? 0 : d.ctl->allCnt;
   if (cnt > d.xAllCap) cnt = 0;  // xPublishAllCount reports the overflow
-  for (int j = VB * blockDim.x + threadIdx.x; j < cnt; j += VG * blockDim.x) xPublishAll(d, j);
-  if (VB == 0 && threadIdx.x == 0) xPublishAllCount(d);
+  for (int j = blk * blockDim.x + threadIdx.x; j < cnt; j += nBlk * blockDim.x) xPublishAll(d, j);
+  if (blk == 0 && threadIdx.x == 0) xPublishAllCount(d);
 }
-__global__ void __launch_bounds__(128) k_x_all_publish(Dev d) { b_x_all_publish(d, blockIdx.x, gridDim.x); }
 // ... and after it every shard builds every sendAll of the pass: the same sorted record in the same slot (replicated records)
-__device__ __forceinline__ void b_x_all_build(const Dev& d, const int VB, const int VG) {
+__global__ void __launch_bounds__(128) k_x_all_build(Dev d) {
   __shared__ int hist[4][ALL_HIST];
   if (d.ctl->error) return;
+  const int blk = blockIdx.x, nBlk = gridDim.x;
   const int cnt = xAllTotal(d);
   const int warp = threadIdx.x >> 5;
   if (warp >= 4) return;
-  const int gw = VB * 4 + warp, nw = VG * 4;
+  const int gw = blk * 4 + warp, nw = nBlk * 4;
   CoopWarp c;
   for (int k = gw; k < cnt; k += nw) xBuildAll(d, c, k, d.allTmp + (size_t)gw * d.N, hist[warp]);
 }
-__global__ void __launch_bounds__(128) k_x_all_build(Dev d) { b_x_all_build(d, blockIdx.x, gridDim.x); }
 
 // ---- multisplit: stable distribution of the new envelopes into the time ring -----------------
 // A block of Dev.msWarps warps handles a chunk of msWarps * MS_SUB consecutive envelopes (creation order); warp w owns the w-th
@@ -539,14 +514,15 @@ __device__ __forceinline__ void msWarpHistogram(const Dev& d, int* hw, int g0, i
   for (int r = 0; r < MS_ROUNDS; ++r)
     if (tg[r] >= 0) atomicAdd(&hw[tg[r] - tick], 1);
 }
-__device__ __forceinline__ void b_ms_count(const Dev& d, const int VB, const int VG) {
+__global__ void __launch_bounds__(256) k_ms_count(Dev d) {
   extern __shared__ int msHist[];  // [msWarps][ring]
   if (d.ctl->error) return;
+  const int blk = blockIdx.x, nBlk = gridDim.x;
   const int G = d.ctl->totalSlots, tick = d.ctl->tick, ring = d.ring;
   const int W = d.msWarps, CH = W * MS_SUB;
   const int nChunks = (G + CH - 1) / CH;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  for (int ch = VB; ch < nChunks; ch += VG) {
+  for (int ch = blk; ch < nChunks; ch += nBlk) {
     msZero(msHist, ring, W);
     __syncthreads();
     int tg[MS_ROUNDS];
@@ -561,15 +537,15 @@ __device__ __forceinline__ void b_ms_count(const Dev& d, const int VB, const int
     __syncthreads();
   }
 }
-__global__ void __launch_bounds__(256) k_ms_count(Dev d) { b_ms_count(d, blockIdx.x, gridDim.x); }
 // per ring bin: running offset over chunks, starting at the bucket's current fill
-__device__ __forceinline__ void b_ms_scan(const Dev& d, const int VB, const int VG) {
+__global__ void k_ms_scan(Dev d) {
   if (d.ctl->error) return;
+  const int blk = blockIdx.x, nBlk = gridDim.x;
   int G = d.ctl->totalSlots, tick = d.ctl->tick, ring = d.ring;
   const int CH = d.msWarps * MS_SUB;
   int nChunks = (G + CH - 1) / CH;
   if (nChunks == 0) return;
-  for (int b = VB * blockDim.x + threadIdx.x; b < ring; b += VG * blockDim.x) {
+  for (int b = blk * blockDim.x + threadIdx.x; b < ring; b += nBlk * blockDim.x) {
     int slot = (tick + b) & (ring - 1);
     int run = d.bucketCount[slot];
     for (int ch0 = 0; ch0 < nChunks; ch0 += 8) {
@@ -590,16 +566,16 @@ __device__ __forceinline__ void b_ms_scan(const Dev& d, const int VB, const int 
     d.bucketCount[slot] = run;
   }
 }
-__global__ void k_ms_scan(Dev d) { b_ms_scan(d, blockIdx.x, gridDim.x); }
-__device__ __forceinline__ void b_ms_scatter(const Dev& d, const int VB, const int VG) {
+__global__ void __launch_bounds__(256) k_ms_scatter(Dev d) {
   extern __shared__ int msHist[];
   if (d.ctl->error) return;
+  const int blk = blockIdx.x, nBlk = gridDim.x;
   const int G = d.ctl->totalSlots, tick = d.ctl->tick, ring = d.ring;
   const int W = d.msWarps, CH = W * MS_SUB;
   const int nChunks = (G + CH - 1) / CH;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   int* base = msHist + warp * ring;
-  for (int ch = VB; ch < nChunks; ch += VG) {
+  for (int ch = blk; ch < nChunks; ch += nBlk) {
     msZero(msHist, ring, W);
     __syncthreads();
     const int g0 = ch * CH + warp * MS_SUB;
@@ -647,136 +623,18 @@ __device__ __forceinline__ void b_ms_scatter(const Dev& d, const int VB, const i
     __syncthreads();
   }
 }
-__global__ void __launch_bounds__(256) k_ms_scatter(Dev d) { b_ms_scatter(d, blockIdx.x, gridDim.x); }
 
-__device__ __forceinline__ void b_free(const Dev& d, const int VB, const int VG) {
+__global__ void k_free(Dev d) {
   if (d.ctl->error) return;
+  const int blk = blockIdx.x, nBlk = gridDim.x;
   const int per = d.freeCap / ARENA_STRIPES;
-  const int stripe = VB & (ARENA_STRIPES - 1);
+  const int stripe = blk & (ARENA_STRIPES - 1);
   int cnt = d.ctl->freeCnt[stripe];
   if (cnt > per) cnt = per;
-  const int sub = (VB >> 6) * blockDim.x + threadIdx.x;
-  const int nsub = (VG >> 6) * blockDim.x;
+  const int sub = (blk >> 6) * blockDim.x + threadIdx.x;
+  const int nsub = (nBlk >> 6) * blockDim.x;
   for (int j = sub; j < cnt; j += nsub) freeApply(d, stripe * per + j);
 }
-__global__ void k_free(Dev d) { b_free(d, blockIdx.x, gridDim.x); }
-
-#if defined(WTG_PERSISTENT_WINDOW)  // experiment kept for reference (DESIGN.md §6): slower than the per-tick graph on an H100 at 16 384 and 65 536 nodes
-// ---- one cooperative kernel per runMs window ------------------------------------------------------------------
-// The pipeline's kernels are tiny at most ticks (a launch boundary costs more than the work), so a whole window runs as
-// ONE cooperative launch: every stage is a grid-stride loop over the virtual blocks of the stage's stand-alone launch
-// configuration, separated by grid-wide barriers instead of kernel boundaries.  Same stage bodies, same order.
-struct RunCfg {
-  int pre0, count1, post2;  // passes: mode 0 (events at the current time), mode 1 (clock ticks), mode 2 (end of window)
-  int sms;
-};
-#define WTG_STAGE(VGRID, CALL)                                        \
-  do {                                                                \
-    const int vg_ = (VGRID);                                          \
-    for (int vb = blockIdx.x; vb < vg_; vb += gridDim.x) { CALL; }    \
-  } while (0)
-__global__ void __launch_bounds__(256) k_run(Dev d, RunCfg rc) {
-  cg::grid_group grid = cg::this_grid();
-  const int total = rc.pre0 + rc.count1 + rc.post2;
-  const int wide = rc.sms * 8;
-  const int striped = ARENA_STRIPES * 19;
-  auto modeOf = [&](int ps) { return ps < rc.pre0 ? 0 : ps < rc.pre0 + rc.count1 ? 1 : 2; };
-  if (blockIdx.x == 0) {
-    if (threadIdx.x == 0) d.ctl->stop = 0;
-    __syncthreads();
-    b_begin(d, modeOf(0), 0, 1);
-  }
-  grid.sync();
-  for (int ps = 0; ps < total; ++ps) {
-    const int mode = modeOf(ps);
-    if (d.proto == PROTO_GSF || d.proto == PROTO_HANDEL) {
-      WTG_STAGE((d.nLoc + 255) / 256, b_cond_mark(d, vb, vg_));
-      grid.sync();
-      WTG_STAGE(striped, b_cond_nodes<0>(d, vb, vg_));
-      grid.sync();
-      WTG_STAGE(striped, b_cond_score(d, vb, vg_));
-      grid.sync();
-      WTG_STAGE(striped, b_cond_nodes<1>(d, vb, vg_));
-      grid.sync();
-      if (d.proto == PROTO_HANDEL) {
-        WTG_STAGE(wide, b_scan_partial(d, 2, vb, vg_));
-        grid.sync();
-        WTG_STAGE(wide, b_scan_final(d, 2, vb, vg_));
-        grid.sync();
-        WTG_STAGE(rc.sms, b_hpick_check(d, vb, vg_));
-        grid.sync();
-        WTG_STAGE(rc.sms, b_hpick_apply(d, vb, vg_));
-        grid.sync();
-      }
-    }
-    if (mode != 2) {
-      WTG_STAGE(wide, b_dispatch_count(d, vb, vg_));
-      grid.sync();
-      WTG_STAGE(wide, b_scan_partial(d, 0, vb, vg_));
-      grid.sync();
-      WTG_STAGE(wide, b_scan_final(d, 0, vb, vg_));
-      grid.sync();
-      WTG_STAGE(wide, b_dispatch_scatter(d, vb, vg_));
-      grid.sync();
-      WTG_STAGE((d.nLoc + 255) / 256, b_node_msgs(d, vb, vg_));
-      grid.sync();
-      WTG_STAGE(striped, b_node_tasks(d, vb, vg_));
-      grid.sync();
-    }
-    WTG_STAGE(wide, b_scan_partial(d, 1, vb, vg_));
-    grid.sync();
-    WTG_STAGE(wide, b_scan_final(d, 1, vb, vg_));
-    grid.sync();
-    if (d.G > 1) {  // node-sharded: exchange 1
-      WTG_STAGE(rc.sms * 2, b_x1_publish(d, vb, vg_));
-      grid.sync();
-      if (blockIdx.x == 0) b_x_sync(d, 0, 0, 1);
-      grid.sync();
-      if (blockIdx.x == 0 && threadIdx.x == 0) b_x1_totals(d, 0, 1);
-      WTG_STAGE(rc.sms * 2, b_x1_offsets(d, vb, vg_));
-      grid.sync();
-    }
-    if (d.shufCap > 0) {
-      WTG_STAGE(ARENA_STRIPES * 4, b_shuffle_check(d, vb, vg_));
-      grid.sync();
-      if (blockIdx.x == 0 && threadIdx.x == 0) b_shuffle_serial(d, 0, 1);
-      grid.sync();
-    }
-    WTG_STAGE(ARENA_STRIPES * 16, b_emit(d, vb, vg_));
-    if (d.allCap > 0) {
-      grid.sync();
-      WTG_STAGE(d.allWarps / 4, b_emit_all(d, vb, vg_));
-    }
-    grid.sync();
-    if (d.G > 1) {  // exchange 2
-      if (blockIdx.x == 0) b_x_sync(d, 1, 0, 1);
-      grid.sync();
-      WTG_STAGE(rc.sms * 4, b_x2_ingest(d, vb, vg_));
-      grid.sync();
-    }
-    WTG_STAGE(rc.sms * 2, b_ms_count(d, vb, vg_));
-    if (d.proto == PROTO_GSF || d.proto == PROTO_HANDEL) WTG_STAGE(ARENA_STRIPES * 2, b_free(d, vb, vg_));
-    grid.sync();
-    WTG_STAGE((d.ring + 255) / 256, b_ms_scan(d, vb, vg_));
-    grid.sync();
-    WTG_STAGE(rc.sms * 2, b_ms_scatter(d, vb, vg_));
-    grid.sync();
-    // end of this pass and beginning of the next, by one warp
-    if (blockIdx.x == 0 && threadIdx.x < 32) {
-      if (threadIdx.x == 0) {
-        tickEnd(d, mode);
-        d.ctl->passesDone += 1;
-        if (d.ctl->error || (d.ffwd && d.ctl->idle)) d.ctl->stop = 1;
-      }
-      __syncwarp();
-      if (ps + 1 < total && !d.ctl->stop) b_begin(d, modeOf(ps + 1), 0, 1);
-    }
-    grid.sync();
-    if (d.ctl->stop) break;
-  }
-}
-
-#endif
 
 // ---- init kernels ---------------------------------------------------------------------------
 __global__ void k_gsf_init_nodes(Dev d) {
@@ -810,8 +668,9 @@ class CudaBackend : public Backend {
   long long launches = 0;      // kernels enqueued (graph replays counted kernel by kernel)
   long long graphKernels = 0;
   cudaEvent_t tm0 = nullptr, tm1 = nullptr;
-  // per-kernel profiling
-  static constexpr int NK = 16;
+  // per-kernel profiling: one slot per timed group of kernels, reported under profNames[slot]
+  enum ProfSlot { P_BEGIN, P_COND_SCAN, P_DISPATCH_COUNT, P_SCAN_PARTIAL, P_EXCHANGE, P_SCAN_FINAL, P_DISPATCH_SCATTER, P_NODE,
+                  P_EMIT, P_MS_COUNT, P_MS_SCAN, P_MS_SCATTER, P_FREE, P_END, P_COND_SCORE, P_COND_SELECT, NK };
   bool profiling = false;
   std::vector<cudaEvent_t> evPool;
   std::vector<int> evKernel;  // kernel id of each event pair
@@ -844,13 +703,8 @@ class CudaBackend : public Backend {
     CUDA_OK(cudaDeviceGetAttribute(&smemOptin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
     CUDA_OK(cudaFuncSetAttribute(k_ms_count, cudaFuncAttributeMaxDynamicSharedMemorySize, smemOptin));
     CUDA_OK(cudaFuncSetAttribute(k_ms_scatter, cudaFuncAttributeMaxDynamicSharedMemorySize, smemOptin));
-    if (NODE_TMA_SMEM > 0) CUDA_OK(cudaFuncSetAttribute(k_node_tasks, cudaFuncAttributeMaxDynamicSharedMemorySize, NODE_TMA_SMEM));
     const char* g = std::getenv("WTG_NO_GRAPH");
     if (g && g[0] == '1') useGraph = false;
-#if defined(WTG_PERSISTENT_WINDOW)
-    const char* np = std::getenv("WTG_NO_PERSIST");
-    if (np && np[0] == '1') usePersistent = false;
-#endif
   }
   ~CudaBackend() override {
     for (void* q : ipcOpened) cudaIpcCloseMemHandle(q);
@@ -890,9 +744,6 @@ class CudaBackend : public Backend {
     std::memcpy(&p, handle + 72, sizeof(p));
     std::memcpy(&dev, handle + 80, 4);
     if (pid == (long long)getpid()) {  // a shard of this process: same address space
-#if defined(WTG_PERSISTENT_WINDOW)
-      if (dev == devId) sharesDevice = true;
-#endif
       if (dev != devId) {
         int can = 0;
         CUDA_OK(cudaDeviceCanAccessPeer(&can, devId, dev));
@@ -1000,78 +851,69 @@ class CudaBackend : public Backend {
     // mode 3: the host prepared the control block and the descriptors of sends it injects at the current time
     // (Engine::inject); only the emission half of the pipeline runs
     if (mode != 3) {
-      profBegin(0);
+      profBegin(P_BEGIN);
       k_begin<<<1, 32, 0, st>>>(d, mode);
       profEnd();
     }
-    if (d.proto == PROTO_HANDEL && mode != 3) {
-      profBegin(1);
+    if ((d.proto == PROTO_GSF || d.proto == PROTO_HANDEL) && mode != 3) {  // conditional tasks (checkSigs)
+      // GSF's select keeps one bit per queue entry per warp in dynamic shared memory; Handel's scratch is static
+      const size_t smem8 = d.proto == PROTO_GSF ? (size_t)8 * (size_t)(d.qcap / 32) * sizeof(uint32_t) : 0;
+      profBegin(P_COND_SCAN);
       k_cond_mark<<<(d.nLoc + 255) / 256, 256, 0, st>>>(d);
       k_cond_nodes<0><<<ARENA_STRIPES * 19, 256, 0, st>>>(d);
       profEnd();
-      profBegin(14);
+      profBegin(P_COND_SCORE);
       k_cond_score<<<ARENA_STRIPES * 19, 256, 0, st>>>(d);
       profEnd();
-      profBegin(15);
-      k_cond_nodes<1><<<ARENA_STRIPES * 19, 256, 0, st>>>(d);
-      profEnd();
-      profBegin(3);
-      k_scan_partial<<<wide, SCAN_THREADS, 0, st>>>(d, 2);
-      profEnd();
-      profBegin(5);
-      k_scan_final<<<wide, SCAN_THREADS, 0, st>>>(d, 2);
-      profEnd();
-      profBegin(15);
-      k_hpick_check<<<sms, 256, 0, st>>>(d);
-      k_hpick_apply<<<sms, 256, 0, st>>>(d);
-      profEnd();
-      launches += 7;
-    }
-    if (d.proto == PROTO_GSF && mode != 3) {
-      size_t smem8 = (size_t)8 * (size_t)(d.qcap / 32) * sizeof(uint32_t);
-      profBegin(1);
-      k_cond_mark<<<(d.nLoc + 255) / 256, 256, 0, st>>>(d);
-      k_cond_nodes<0><<<ARENA_STRIPES * 19, 256, 0, st>>>(d);
-      profEnd();
-      profBegin(14);
-      k_cond_score<<<ARENA_STRIPES * 19, 256, 0, st>>>(d);
-      profEnd();
-      profBegin(15);
+      profBegin(P_COND_SELECT);
       k_cond_nodes<1><<<ARENA_STRIPES * 19, 256, smem8, st>>>(d);
       profEnd();
       launches += 4;
+      if (d.proto == PROTO_HANDEL) {  // draw scan and pick
+        profBegin(P_SCAN_PARTIAL);
+        k_scan_partial<<<wide, SCAN_THREADS, 0, st>>>(d, 2);
+        profEnd();
+        profBegin(P_SCAN_FINAL);
+        k_scan_final<<<wide, SCAN_THREADS, 0, st>>>(d, 2);
+        profEnd();
+        profBegin(P_COND_SELECT);
+        k_hpick_check<<<sms, 256, 0, st>>>(d);
+        k_hpick_apply<<<sms, 256, 0, st>>>(d);
+        profEnd();
+        launches += 3;
+      }
     }
-    if (mode != 2 && mode != 3) {
-      profBegin(2);
-    k_dispatch_count<<<wide, 256, 0, st>>>(d);
-    profEnd();
-      profBegin(3);
-    k_scan_partial<<<wide, SCAN_THREADS, 0, st>>>(d, 0);
-    profEnd();
-      profBegin(5);
-    k_scan_final<<<wide, SCAN_THREADS, 0, st>>>(d, 0);
-    profEnd();
-      profBegin(6);
-    k_dispatch_scatter<<<wide, 256, 0, st>>>(d);
-    profEnd();
-      profBegin(7);
-    k_node_msgs<<<(d.nLoc + 255) / 256, 256, 0, st>>>(d);
-    k_node_tasks<<<ARENA_STRIPES * 19, 256, NODE_TMA_SMEM, st>>>(d);
-    if (d.proto == PROTO_CASPER) {
-      k_casper_fixups<<<1, 32, 0, st>>>(d);
-      launches += 1;
-    }
-    profEnd();
+    if (mode != 2 && mode != 3) {  // dispatch and handlers
+      profBegin(P_DISPATCH_COUNT);
+      k_dispatch_count<<<wide, 256, 0, st>>>(d);
+      profEnd();
+      profBegin(P_SCAN_PARTIAL);
+      k_scan_partial<<<wide, SCAN_THREADS, 0, st>>>(d, 0);
+      profEnd();
+      profBegin(P_SCAN_FINAL);
+      k_scan_final<<<wide, SCAN_THREADS, 0, st>>>(d, 0);
+      profEnd();
+      profBegin(P_DISPATCH_SCATTER);
+      k_dispatch_scatter<<<wide, 256, 0, st>>>(d);
+      profEnd();
+      profBegin(P_NODE);
+      k_node_msgs<<<(d.nLoc + 255) / 256, 256, 0, st>>>(d);
+      k_node_tasks<<<ARENA_STRIPES * 19, 256, 0, st>>>(d);
+      if (d.proto == PROTO_CASPER) {
+        k_casper_fixups<<<1, 32, 0, st>>>(d);
+        launches += 1;
+      }
+      profEnd();
       launches += 6;
     }
-    profBegin(3);
+    profBegin(P_SCAN_PARTIAL);
     k_scan_partial<<<wide, SCAN_THREADS, 0, st>>>(d, 1);
     profEnd();
-    profBegin(5);
+    profBegin(P_SCAN_FINAL);
     k_scan_final<<<wide, SCAN_THREADS, 0, st>>>(d, 1);
     profEnd();
     if (d.G > 1) {  // node-sharded: exchange 1 (items -> creation / draw offsets over all shards)
-      profBegin(4);
+      profBegin(P_EXCHANGE);
       k_x1_publish<<<sms * 2, 256, 0, st>>>(d);
       k_x_sync<<<1, 32, 0, st>>>(d, 0);
       k_x1_totals<<<1, 1, 0, st>>>(d);
@@ -1079,7 +921,7 @@ class CudaBackend : public Backend {
       profEnd();
       launches += 4;
     }
-    profBegin(8);
+    profBegin(P_EMIT);
     if (d.shufCap > 0) {
       k_shuffle_check<<<ARENA_STRIPES * 4, 256, 0, st>>>(d);
       k_shuffle_serial<<<1, 1, 0, st>>>(d);
@@ -1095,7 +937,7 @@ class CudaBackend : public Backend {
     }
     profEnd();
     if (d.G > 1) {  // exchange 2: the envelopes were stored into their destination shards' arrays by k_emit
-      profBegin(4);
+      profBegin(P_EXCHANGE);
       k_x_sync<<<1, 32, 0, st>>>(d, 1);
       k_x2_ingest<<<sms * 4, 256, 0, st>>>(d);
       launches += 2;
@@ -1105,69 +947,26 @@ class CudaBackend : public Backend {
       }
       profEnd();
     }
-    profBegin(9);
+    profBegin(P_MS_COUNT);
     k_ms_count<<<sms * 2, d.msWarps * 32, msSmem, st>>>(d);
     profEnd();
-    profBegin(10);
+    profBegin(P_MS_SCAN);
     k_ms_scan<<<(d.ring + 127) / 128, 128, 0, st>>>(d);
     profEnd();
-    profBegin(11);
+    profBegin(P_MS_SCATTER);
     k_ms_scatter<<<sms * 2, d.msWarps * 32, msSmem, st>>>(d);
     profEnd();
     const bool pooled = d.proto == PROTO_GSF || d.proto == PROTO_HANDEL;  // only these protocols hold pooled payloads
     if (pooled) {
-      profBegin(12);
+      profBegin(P_FREE);
       k_free<<<ARENA_STRIPES * 2, 256, 0, st>>>(d);
       profEnd();
     }
-    profBegin(13);
+    profBegin(P_END);
     k_end<<<1, 1, 0, st>>>(d, mode);
     profEnd();
     launches += pooled ? 9 : 8;
   }
-#if defined(WTG_PERSISTENT_WINDOW)
-  // ---- one cooperative launch per window (k_run) ----
-  bool usePersistent = true;
-  bool sharesDevice = false;   // another shard of this process lives on this GPU: two cooperative grids that wait for each
-                               // other cannot be co-resident, so such shards keep the kernel-per-stage pipeline
-  int runGrid = 0;
-  size_t runSmem = 0;
-  const void* runFor = nullptr;
-  long long windows = 0;
-  bool persistentOk(const Dev& d) {
-    if (!usePersistent || profiling || sharesDevice) return false;
-    size_t need = std::max((size_t)8 * d.ring * sizeof(int), (size_t)8 * (size_t)(d.qcap / 32 + 1) * sizeof(uint32_t));
-    if (need > 200 * 1024) return false;
-    if (runFor != (const void*)d.ctl || runSmem != need) {
-      CUDA_OK(cudaFuncSetAttribute(k_run, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)need));
-      int per = 0;
-      CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per, k_run, 256, need));
-      if (per < 1) return false;
-      const char* cap = std::getenv("WTG_RUN_BLOCKS_PER_SM");
-      if (cap && std::atoi(cap) > 0) per = std::min(per, std::atoi(cap));
-      runGrid = per * sms;
-      runSmem = need;
-      runFor = (const void*)d.ctl;
-    }
-    return true;
-  }
-  void runWindow(const Dev& d, int pre0, int count1, int post2) override {
-    bind();
-    if (pre0 + count1 + post2 <= 0) return;
-    if (!persistentOk(d)) {
-      if (pre0) tick(d, 0);
-      if (count1) ticks(d, count1);
-      if (post2) tick(d, 2);
-      return;
-    }
-    RunCfg rc{pre0, count1, post2, sms};
-    Dev dd = d;
-    void* args[] = {(void*)&dd, (void*)&rc};
-    CUDA_OK(cudaLaunchCooperativeKernel((const void*)k_run, dim3(runGrid), dim3(256), args, runSmem, st));
-    launches += 1;
-    windows += 1;
-  }
-#endif
   // dynamic shared memory of the multisplit kernels: the attribute is per device and shared by every engine on it (several
   // engines may be driven from concurrent host threads), so it is set once, to the device's opt-in maximum
   void configure(const Dev& d) {

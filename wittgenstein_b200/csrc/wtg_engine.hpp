@@ -66,13 +66,6 @@ struct Backend {
   virtual void ticks(const Dev& d, int count) {
     for (int i = 0; i < count; ++i) tick(d, 1);
   }
-  // a whole runMs window: pre0 passes of mode 0, count1 clock ticks, post2 end-of-window passes.  A pass loop may stop early
-  // when the device reports an error or (fast-forwarding protocols) that nothing is left before `until`.
-  virtual void runWindow(const Dev& d, int pre0, int count1, int post2) {
-    if (pre0) tick(d, 0);
-    if (count1) ticks(d, count1);
-    if (post2) tick(d, 2);
-  }
   // device-side timing (CUDA events on the engine's stream); no-ops on backends without a device
   virtual void timerStart() {}
   virtual double timerStopMs() { return 0.0; }
@@ -1399,7 +1392,7 @@ class Engine {
       for (long long done = 0;;) {
         int batch = (int)std::min<long long>(grow, std::max<long long>(1, ms - done));
         if (grow < 64) grow *= 2;  // busy windows: fewer host round trips
-        be->runWindow(d, 0, batch, 0);
+        runWindow(0, batch, 0);
         done += batch;
         c = readCtl();
         if (c.error) throwDeviceError(c);
@@ -1411,7 +1404,7 @@ class Engine {
       return c.didSomething ? 1 : 0;
     }
     writeCtl(c);
-    be->runWindow(d, pendingAtNow ? 1 : 0, ms, 1);
+    runWindow(pendingAtNow ? 1 : 0, ms, 1);
     pendingAtNow = false;
     c = readCtl();
     if (c.error) throwDeviceError(c);
@@ -1639,6 +1632,14 @@ class Engine {
   void fetch(T* out, const T* dev, size_t n) {
     be->sync();
     be->download(out, dev, n * sizeof(T));
+  }
+
+ private:
+  // a whole runMs window: pre0 passes of mode 0, count1 clock ticks, post2 end-of-window passes
+  void runWindow(int pre0, int count1, int post2) {
+    if (pre0) be->tick(d, 0);
+    if (count1) be->ticks(d, count1);
+    if (post2) be->tick(d, 2);
   }
 };
 

@@ -18,7 +18,6 @@
 //   protocols/PingPong.java:60-87                                        -> ppDeliver
 #pragma once
 #include "wtg_types.h"
-#include "wtg_tma.cuh"
 
 // host stand-ins (single-threaded debugging build / nvcc host pass of __host__ __device__ bodies)
 template <class T, class U>
@@ -93,7 +92,6 @@ struct CoopWarp {
   __device__ __forceinline__ u64 bcast64(u64 v, int src) const { return __shfl_sync(0xffffffffu, v, src); }
   __device__ __forceinline__ void sync() const { __syncwarp(); }
   __device__ __forceinline__ int gather(int mine, int src, const int*) const { return __shfl_sync(0xffffffffu, mine, src); }
-  TmaWarp tma;  // bulk-copy tiles of this warp (kernels that snapshot payloads set it up; buf == nullptr: none)
 };
 #endif
 
@@ -1196,68 +1194,15 @@ __device__ __forceinline__ void gsfCycleWarp(const Dev& d, CoopWarp& c, int n, i
   }
   unsigned pm = __ballot_sync(FULLM, pooled);
   unsigned long long words = 0;
-#if defined(WTG_TMA_SNAPSHOT)  // experiment kept for reference (DESIGN.md §6): slower than the lane-strided copy on an H100
-  if (pm && c.tma.buf != nullptr) {
-    // The snapshots of all sending levels are nested sub-ranges of ONE range of the row: the block of the highest sending
-    // level (every level block contains n).  It is read once, by bulk asynchronous copies into this warp's shared-memory
-    // tiles (4 KiB batches), and every level's slab is written from there by bulk stores (wtg_tma.cuh).
-    const int top = 31 - __clz(pm);
-    const Blk tb = levelBlock(n, top);
-    const uint32_t topBytes = (uint32_t)tb.nw * 8u;
-    const uint32_t BATCH = (uint32_t)(TMA_TILES * TMA_TILE_BYTES);
-    for (uint32_t off = 0; off < topBytes; off += BATCH) {
-      const uint32_t len = topBytes - off < BATCH ? topBytes - off : BATCH;
-      // does any level's block intersect this batch?  (lower levels lie in one aligned part of the top block)
-      unsigned m = pm;
-      bool any = false;
-      while (m) {
-        const int src = __ffs(m) - 1;
-        m &= m - 1;
-        const Blk ob = levelBlock(n, src);
-        const uint32_t lo = (uint32_t)(ob.w0 - tb.w0) * 8u, hi = lo + (uint32_t)ob.nw * 8u;
-        any |= lo < off + len && hi > off;
-      }
-      if (!any) continue;
-      if (lane == 0) tmaLoadLane(c.tma, rowV + tb.w0 + off / 8u, len);
-      m = pm;
-      while (m) {
-        const int src = __ffs(m) - 1;
-        m &= m - 1;
-        const uint32_t sl = __shfl_sync(FULLM, slot, src);
-        const int so = __shfl_sync(FULLM, stagedOn, src);
-        const Blk ob = levelBlock(n, src);
-        const uint32_t lo = (uint32_t)(ob.w0 - tb.w0) * 8u, hi = lo + (uint32_t)ob.nw * 8u;
-        const uint32_t a = lo > off ? lo : off, e = hi < off + len ? hi : off + len;
-        if (a < e && lane == 0) {
-          u64* dstp = so >= 0 ? xStagePtr(d, so, d.rank, (int)sl) : d.pool[src] + (size_t)sl * (size_t)ob.nw;
-          bulkStore(dstp + (a - lo) / 8u, c.tma.buf + (a - off) / 8u, e - a);
-        }
-      }
-      if (lane == 0) {
-        bulkCommit();
-        bulkWaitRead0();  // the tiles are free again
-      }
-    }
-    unsigned m2 = pm;
-    while (m2) {
-      const int src = __ffs(m2) - 1;
-      m2 &= m2 - 1;
-      words += (unsigned long long)(2 * levelBlock(n, src).nw);
-    }
-    __syncwarp();
-  } else
-#endif
-  {
-    while (pm) {
-      int src = __ffs(pm) - 1;
-      pm &= pm - 1;
-      uint32_t sl = __shfl_sync(FULLM, slot, src);
-      int so = __shfl_sync(FULLM, stagedOn, src);
-      Blk ob = levelBlock(n, src);  // our own half of level `src`: what the receiver waits for at its level
-      u64* dstp = so >= 0 ? xStagePtr(d, so, d.rank, (int)sl) : d.pool[src] + (size_t)sl * (size_t)ob.nw;
-      warpCopyWords(dstp, rowV + ob.w0, ob.nw, lane);
-      words += (unsigned long long)(2 * ob.nw);
-    }
+  while (pm) {
+    int src = __ffs(pm) - 1;
+    pm &= pm - 1;
+    uint32_t sl = __shfl_sync(FULLM, slot, src);
+    int so = __shfl_sync(FULLM, stagedOn, src);
+    Blk ob = levelBlock(n, src);  // our own half of level `src`: what the receiver waits for at its level
+    u64* dstp = so >= 0 ? xStagePtr(d, so, d.rank, (int)sl) : d.pool[src] + (size_t)sl * (size_t)ob.nw;
+    warpCopyWords(dstp, rowV + ob.w0, ob.nw, lane);
+    words += (unsigned long long)(2 * ob.nw);
   }
   if (snd && base >= 0) {
     Desc ds;

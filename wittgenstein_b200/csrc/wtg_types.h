@@ -202,8 +202,6 @@ struct Ctl {  // device-resident control block (one per engine)
   int tick;       // tick being processed
   int condMode;   // 0 = no conditional-task pass, 1 = normal, 2 = end-of-window overshoot pass
   int nEv;        // events in this tick's bucket
-  int nDesc;      // (unused) total descriptors; per-stripe counts below
-  int nDestScratch;
   int nItems;     // scan items this tick (N + nEv)
   int totalSlots, totalDraws;
   uint32_t callId;  // identity of the reference's current nextMessage() call (conditional-task snapshot)
@@ -227,8 +225,6 @@ struct Ctl {  // device-resident control block (one per engine)
   int dueCnt[ARENA_STRIPES];    // nodes whose conditional task runs this tick, per stripe
   int taskCnt[ARENA_STRIPES];   // nodes with task events this tick, per stripe
   // ---- node-sharded simulation ----
-  int stop;                      // persistent window kernel: leave the pass loop (error, or nothing left to do)
-  int passesDone;                // passes completed by window kernels (statistics)
   int xseq;                      // pipeline passes so far (identical on every shard): sequence number of the exchanges
   int nEvGlobal;                 // bucket entries of this tick over all shards
   int condXoffS, condXoffD;      // creation / draw index of this shard's first conditional-task insert
