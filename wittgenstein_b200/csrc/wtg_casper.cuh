@@ -14,12 +14,6 @@
 
 namespace wtg {
 
-#if defined(__CUDA_ARCH__)
-#define WTG_CTZ64(x) (__ffsll((long long)(x)) - 1)
-#else
-#define WTG_CTZ64(x) __builtin_ctzll(x)
-#endif
-
 struct CMask {  // a set of blocks
   u64 w[CASPER_MAX_BLKWORDS];
 };
@@ -777,51 +771,17 @@ WTG_HD void emitAllCore(const Dev& d, C& c, uint32_t fromU, uint32_t meta, u64 p
         }
         c.sync();
         int run = placed;  // exclusive prefix over the arrival bins
-#if defined(__CUDA_ARCH__)
-        if (C::LANES == 32) {
-          for (int b0 = 0; b0 < ALL_HIST; b0 += 32) {
-            int v = hist[b0 + c.lane()], inc = v;
-#pragma unroll
-            for (int o = 1; o < 32; o <<= 1) {
-              int t = __shfl_up_sync(0xffffffffu, inc, o);
-              if (c.lane() >= o) inc += t;
-            }
-            hist[b0 + c.lane()] = run + inc - v;
-            run += __shfl_sync(0xffffffffu, inc, 31);
-          }
-        } else
-#endif
-        {
-          for (int b = 0; b < ALL_HIST; ++b) {
-            int v = hist[b];
-            hist[b] = run;
-            run += v;
-          }
+        for (int b0 = 0; b0 < ALL_HIST; b0 += C::LANES) {
+          int total;
+          hist[b0 + c.lane()] = run + c.exclusiveScan(hist[b0 + c.lane()], total);
+          run += total;
         }
         c.sync();
         for (int to0 = 0; to0 < N; to0 += C::LANES) {  // stable: destinations in id order, LANES at a time
           int to = to0 + c.lane();
           int a = to < N ? tmp[to] : -1;
           bool in = a >= base && a < base + ALL_HIST;
-          int pos = 0;
-#if defined(__CUDA_ARCH__)
-          if (C::LANES == 32) {
-            int bin = in ? a - base : -1 - c.lane();
-            unsigned peers = __match_any_sync(0xffffffffu, bin);
-            int rank = __popc(peers & ((1u << c.lane()) - 1u));
-            int leader = __ffs(peers) - 1;
-            int b0 = 0;
-            if (in && c.lane() == leader) {
-              b0 = hist[bin];
-              hist[bin] = b0 + __popc(peers);
-            }
-            b0 = __shfl_sync(0xffffffffu, b0, leader);
-            pos = b0 + rank;
-          } else
-#endif
-          {
-            if (in) pos = hist[a - base]++;
-          }
+          int pos = c.claim(hist, a - base, in);
           if (in) {
             d.recDest[off + pos] = (uint32_t)to;
             d.recArrival[off + pos] = a;
@@ -954,19 +914,8 @@ WTG_HD void farMigrate(const Dev& d, C& c, int t) {
     int i = i0 + c.lane();
     bool sel = i < cnt && d.far[i].target <= limit;
     uint32_t m = c.ballot(sel);
-    if (sel) {
-#if defined(__CUDA_ARCH__)
-      int off = C::LANES == 32 ? __popc(m & ((1u << c.lane()) - 1u)) : 0;
-#else
-      int off = 0;
-#endif
-      d.farSel[nsel + off] = i;
-    }
-#if defined(__CUDA_ARCH__)
-    nsel += C::LANES == 32 ? __popc(m) : (int)(m & 1u);
-#else
-    nsel += (int)(m & 1u);
-#endif
+    if (sel) d.farSel[nsel + c.rank(m)] = i;
+    nsel += c.count(m);
   }
   c.sync();
   for (int s = c.lane(); s < nsel; s += C::LANES) {
@@ -1004,19 +953,10 @@ WTG_HD void farMigrate(const Dev& d, C& c, int t) {
     uint32_t m = c.ballot(live);
     c.sync();
     if (live) {
-#if defined(__CUDA_ARCH__)
-      int off = C::LANES == 32 ? __popc(m & ((1u << c.lane()) - 1u)) : 0;
-#else
-      int off = 0;
-#endif
-      d.far[kept + off] = e;
+      d.far[kept + c.rank(m)] = e;
       mn = e.target < mn ? e.target : mn;
     }
-#if defined(__CUDA_ARCH__)
-    kept += C::LANES == 32 ? __popc(m) : (int)(m & 1u);
-#else
-    kept += (int)(m & 1u);
-#endif
+    kept += c.count(m);
     c.sync();
   }
   mn = c.minv(mn);

@@ -47,34 +47,20 @@ __global__ void k_end(Dev d, int mode) {
 }
 
 // ---- conditional tasks (checkSigs): scan -> score -> select ---------------------------------------
-// append node n to a striped list (stripe = global warp index & 63; a stripe receives at most listStripeCap nodes)
-__device__ __forceinline__ void listAppend(const Dev& d, bool active, int n, int* cnt, int* list) {
-  unsigned m = __ballot_sync(0xffffffffu, active);
+// append node n to a striped list (stripe = global warp index & 63; a stripe receives at most listStripeCap nodes),
+// with a 64-bit payload per entry when `words` is given
+__device__ __forceinline__ void listAppend(const Dev& d, bool active, int n, int* cnt, int* list, u64* words = nullptr, u64 word = 0) {
+  CoopWarp c;
+  unsigned m = c.ballot(active);
   if (!m) return;
-  int lane = threadIdx.x & 31;
-  const int blk = blockIdx.x;
-  int gw = (blk * blockDim.x + threadIdx.x) >> 5;
-  int stripe = gw & (ARENA_STRIPES - 1);
+  int stripe = ((blockIdx.x * blockDim.x + threadIdx.x) >> 5) & (ARENA_STRIPES - 1);
   int base = 0;
-  if (lane == 0) base = atomicAdd(&cnt[stripe], __popc(m));
-  base = __shfl_sync(0xffffffffu, base, 0);
-  if (active) list[(size_t)stripe * d.listStripeCap + base + __popc(m & ((1u << lane) - 1u))] = n;
-}
-// same, with a 64-bit payload per entry
-__device__ __forceinline__ void listAppendW(const Dev& d, bool active, int n, u64 word, int* cnt, int* list, u64* words) {
-  unsigned m = __ballot_sync(0xffffffffu, active);
-  if (!m) return;
-  int lane = threadIdx.x & 31;
-  const int blk = blockIdx.x;
-  int gw = (blk * blockDim.x + threadIdx.x) >> 5;
-  int stripe = gw & (ARENA_STRIPES - 1);
-  int base = 0;
-  if (lane == 0) base = atomicAdd(&cnt[stripe], __popc(m));
-  base = __shfl_sync(0xffffffffu, base, 0);
+  if (c.lane() == 0) base = atomicAdd(&cnt[stripe], c.count(m));
+  base = c.bcast(base, 0);
   if (active) {
-    size_t at = (size_t)stripe * d.listStripeCap + base + __popc(m & ((1u << lane) - 1u));
+    size_t at = (size_t)stripe * d.listStripeCap + base + c.rank(m);
     list[at] = n;
-    words[at] = word;
+    if (words) words[at] = word;
   }
 }
 // conditional-task bookkeeping, one thread per node -> list of due nodes
@@ -217,7 +203,7 @@ __global__ void __launch_bounds__(256) k_node_msgs(Dev d) {
     } else
       flag = 1;
   }
-  listAppendW(d, flag != 0, n, word, d.ctl->taskCnt, d.taskList, d.taskWord);
+  listAppend(d, flag != 0, n, d.ctl->taskCnt, d.taskList, d.taskWord, word);
 }
 // pass 2: one warp per node that has tasks (updateVerifiedSignatures / doCycle / ...), or, for protocols whose
 // events do not commute (Handel), all of the node's events in reference order; blocks assigned to list stripes.
@@ -429,13 +415,12 @@ __global__ void __launch_bounds__(256) k_x2_ingest(Dev d) {
   const int blk = blockIdx.x, nBlk = gridDim.x;
   const int G = d.ctl->totalSlots;
   CoopWarp c;
-  const int lane = threadIdx.x & 31;
   const int gw = (blk * blockDim.x + threadIdx.x) >> 5, nw = (nBlk * blockDim.x) >> 5;
   for (int g0 = gw * 32; g0 < G; g0 += nw * 32) {
-    int g = g0 + lane;
-    unsigned m = __ballot_sync(0xffffffffu, g < G && xNeedsIngest(d, g));
+    int g = g0 + c.lane();
+    unsigned m = c.ballot(g < G && xNeedsIngest(d, g));
     while (m) {
-      int src = __ffs(m) - 1;
+      int src = c.first(m);
       m &= m - 1;
       xIngest(d, c, g0 + src);
     }
@@ -575,6 +560,7 @@ __global__ void __launch_bounds__(256) k_ms_scatter(Dev d) {
   const int nChunks = (G + CH - 1) / CH;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   int* base = msHist + warp * ring;
+  CoopWarp cw;
   for (int ch = blk; ch < nChunks; ch += nBlk) {
     msZero(msHist, ring, W);
     __syncthreads();
@@ -596,18 +582,8 @@ __global__ void __launch_bounds__(256) k_ms_scatter(Dev d) {
     for (int r = 0; r < MS_ROUNDS; ++r) {
       int g = g0 + r * 32 + lane;
       int t = tg[r];
-      int bin = t >= 0 ? t - tick : -1 - lane;  // unique negative key for lanes without an envelope
-      unsigned peers = __match_any_sync(0xffffffffu, bin);
-      int rank = __popc(peers & ((1u << lane) - 1u));
-      int leader = __ffs(peers) - 1;
-      int b0 = 0;
-      if (t >= 0 && lane == leader) {
-        b0 = base[bin];
-        base[bin] = b0 + __popc(peers);
-      }
-      b0 = __shfl_sync(0xffffffffu, b0, leader);
+      int pos = cw.claim(base, t - tick, t >= 0);
       if (t >= 0) {
-        int pos = b0 + rank;
         if (pos < d.bcap) {
           const int4* src = reinterpret_cast<const int4*>(d.newEv + g);
           int4* dst = reinterpret_cast<int4*>(d.buckets + (size_t)(t & (ring - 1)) * (size_t)d.bcap + pos);

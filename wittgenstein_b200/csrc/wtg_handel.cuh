@@ -230,11 +230,7 @@ WTG_HD void hDissemination(const Dev& d, C& c, int n, int item, int& outSlots, i
       prefix += d.hCntInc[n * L + l];
     }
   }
-#if defined(__CUDA_ARCH__)
-  int nSend = __popc(sendMask);
-#else
-  int nSend = __builtin_popcount(sendMask);
-#endif
+  int nSend = WTG_POPC32(sendMask);
   int base = descAlloc(d, c, n, nSend + 1);
   int sub = 0;
   long long bytes = 0;
@@ -323,13 +319,7 @@ WTG_HD void hUpdate(const Dev& d, C& c, int n, uint32_t from, uint32_t meta, u64
       int i = base + c.lane();
       bool hit = i < len && q[i].id == id;
       uint32_t m = c.ballot(hit);
-      if (m) {
-#if defined(__CUDA_ARCH__)
-        found = base + __ffs(m) - 1;
-#else
-        found = base;
-#endif
-      }
+      if (m) found = base + c.first(m);
     }
     if (found >= 0) {
       for (int base = found; base < len - 1; base += C::LANES) {
@@ -556,11 +546,7 @@ WTG_HD void hCondScanQueue(const Dev& d, C& c, int n) {
     }
     uint32_t pm = c.ballot(stalePool);
     if (pm) {
-#if defined(__CUDA_ARCH__)
-      int cnt = __popc(pm), off = __popc(pm & ((1u << c.lane()) - 1u));
-#else
-      int cnt = (int)(pm & 1u), off = 0;
-#endif
+      int cnt = c.count(pm), off = c.rank(pm);
       int b0 = 0;
       if (c.lane() == 0) b0 = WTG_ATOMIC_ADD(&d.ctl->workCnt[st], cnt);
       b0 = c.bcast(b0, 0);
@@ -626,10 +612,9 @@ WTG_HD void hCondSelect(const Dev& d, C& c, int n, HScratch* sc) {
   // One lane per level first answers the common case from cached state: the peer at the old index is still a
   // candidate (so suicideBizAfter does not move) and the level's cached minimum rank says nobody is below maxRank.
   // Only the levels that need a walk of the emission list take the cooperative path below.
-  uint32_t slowLevels = 0xFFFFFFFEu;
-#if defined(__CUDA_ARCH__)
-  if (C::LANES == 32) {
-    const int l = c.lane();
+  uint32_t slowLevels = 0;
+  for (int k = 0; k < 32 / C::LANES; ++k) {  // levels as lanes (see gsfLastFinishedLevel)
+    const int l = k * C::LANES + c.lane();
     bool slow = false;
     if (l >= 1 && l < L && sc->count[l] > 0) {
       int biz = d.hBiz[n * L + l];
@@ -639,9 +624,8 @@ WTG_HD void hCondSelect(const Dev& d, C& c, int n, HScratch* sc) {
         slow = !(d.ndown[p] && !rowBit(blRow, p)) || bmin == (-2147483647 - 1) || sc->minRank[l] + window > bmin;
       }
     }
-    slowLevels = c.ballot(slow);
+    slowLevels |= c.ballot(slow) << (k * C::LANES);
   }
-#endif
   for (int l = 1; l < L; ++l) {
     if (!((slowLevels >> l) & 1u)) continue;
     int biz = d.hBiz[n * L + l];
@@ -657,13 +641,7 @@ WTG_HD void hCondSelect(const Dev& d, C& c, int n, HScratch* sc) {
         cand = d.ndown[p] && !rowBit(blRow, p);
       }
       uint32_t m = c.ballot(cand);
-      if (m) {
-#if defined(__CUDA_ARCH__)
-        first = base + __ffs(m) - 1;
-#else
-        first = base;
-#endif
-      }
+      if (m) first = base + c.first(m);
     }
     int hitP = -1, hitR = 0;
     if (first >= 0) {
@@ -695,11 +673,7 @@ WTG_HD void hCondSelect(const Dev& d, C& c, int n, HScratch* sc) {
             }
             uint32_t m = c.ballot(hit);
             if (m && hitP < 0) {
-#if defined(__CUDA_ARCH__)
-              int src = __ffs(m) - 1;
-#else
-              int src = 0;
-#endif
+              int src = c.first(m);
               hitP = c.bcast(pp[u], src);
               hitR = c.bcast(rr[u], src);
             }
@@ -726,11 +700,7 @@ WTG_HD void hCondSelect(const Dev& d, C& c, int n, HScratch* sc) {
           for (int u = 0; u < FU; ++u) {
             uint32_t m = c.ballot(cc[u] && rr[u] < maxRank);
             if (m && hitP < 0) {
-#if defined(__CUDA_ARCH__)
-              int src = __ffs(m) - 1;
-#else
-              int src = 0;
-#endif
+              int src = c.first(m);
               hitP = c.bcast(pp[u], src);
               hitR = c.bcast(rr[u], src);
             }
@@ -768,11 +738,7 @@ WTG_HD void hCondSelect(const Dev& d, C& c, int n, HScratch* sc) {
     }
     uint32_t km = c.ballot(keep);
     c.sync();
-#if defined(__CUDA_ARCH__)
-    int off = __popc(km & ((1u << c.lane()) - 1u)), tot = __popc(km);
-#else
-    int off = 0, tot = (int)(km & 1u);
-#endif
+    int off = c.rank(km), tot = c.count(km);
     if (keep && w + off != i) {
       q[w + off] = e;
       qst[w + off] = st;

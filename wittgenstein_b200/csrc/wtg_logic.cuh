@@ -14,7 +14,7 @@
 //   protocols/GSFSignature.java:557-583 checkSigs                        -> gsfCheckSigs
 //   protocols/GSFSignature.java:537-555 onNewSig                         -> gsfOnNewSig
 //   protocols/GSFSignature.java:384-460 updateVerifiedSignatures         -> gsfUpdate
-//   protocols/GSFSignature.java:212-224, 313-349 doCycle/getRemainingPeers -> gsfCycle
+//   protocols/GSFSignature.java:212-224, 313-349 doCycle/getRemainingPeers -> gsfDoCycle
 //   protocols/PingPong.java:60-87                                        -> ppDeliver
 #pragma once
 #include "wtg_types.h"
@@ -50,12 +50,18 @@ static inline T wtg_host_cas(T* p, T a, T b) {
 #define WTG_ATOMIC_MIN(p, v) atomicMin((p), (v))
 #define WTG_ATOMIC_CAS(p, a, b) atomicCAS((p), (a), (b))
 #define WTG_POPC64(x) __popcll(x)
+#define WTG_POPC32(x) __popc(x)
+#define WTG_CTZ32(x) (__ffs((int)(x)) - 1)
+#define WTG_CTZ64(x) (__ffsll((long long)(x)) - 1)
 #else
 #define WTG_ATOMIC_ADD(p, v) wtg_host_fetch_add((p), (v))
 #define WTG_ATOMIC_MAX(p, v) wtg_host_fetch_max((p), (v))
 #define WTG_ATOMIC_MIN(p, v) wtg_host_fetch_min((p), (v))
 #define WTG_ATOMIC_CAS(p, a, b) wtg_host_cas((p), (a), (b))
 #define WTG_POPC64(x) __builtin_popcountll(x)
+#define WTG_POPC32(x) __builtin_popcount(x)
+#define WTG_CTZ32(x) __builtin_ctz(x)
+#define WTG_CTZ64(x) __builtin_ctzll(x)
 #endif
 
 namespace wtg {
@@ -78,12 +84,64 @@ struct CoopSerial {
   WTG_HD void sync() const {}
   // value held by lane `src` of a per-lane table (serial: read the table itself)
   WTG_HD int gather(int, int src, const int* table) const { return table[src]; }
+  // of a ballot m: lanes set, lanes set below this one, lowest lane set (m != 0)
+  WTG_HD int count(uint32_t m) const { return (int)(m & 1u); }
+  WTG_HD int rank(uint32_t) const { return 0; }
+  WTG_HD int first(uint32_t) const { return 0; }
+  // sum of v over the lanes below this one; total = sum over all lanes
+  WTG_HD int exclusiveScan(int v, int& total) const {
+    total = v;
+    return 0;
+  }
+  // next slot of bins[bin] for every active lane, in lane order
+  WTG_HD int claim(int* bins, int bin, bool active) const { return active ? bins[bin]++ : 0; }
+  // copy a level block of nw words (nw even, both sides 16-byte aligned)
+  WTG_HD void copyWords(u64* dst, const u64* src, int nw) const {
+    for (int w = 0; w < nw; ++w) dst[w] = src[w];
+  }
 };
 #if defined(__CUDACC__)
 struct CoopWarp {
   static constexpr int LANES = 32;
   __device__ __forceinline__ int lane() const { return threadIdx.x & 31; }
   __device__ __forceinline__ uint32_t ballot(bool p) const { return __ballot_sync(0xffffffffu, p); }
+  __device__ __forceinline__ int count(uint32_t m) const { return __popc(m); }
+  __device__ __forceinline__ int rank(uint32_t m) const { return __popc(m & ((1u << lane()) - 1u)); }
+  __device__ __forceinline__ int first(uint32_t m) const { return __ffs(m) - 1; }
+  __device__ __forceinline__ int exclusiveScan(int v, int& total) const {
+    int inc = v;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      int t = __shfl_up_sync(0xffffffffu, inc, o);
+      if (lane() >= o) inc += t;
+    }
+    total = __shfl_sync(0xffffffffu, inc, 31);
+    return inc - v;
+  }
+  __device__ __forceinline__ int claim(int* bins, int bin, bool active) const {
+    const unsigned peers = __match_any_sync(0xffffffffu, active ? bin : -1 - lane());  // inactive lanes: a key of their own
+    const int leader = __ffs(peers) - 1;
+    int b0 = 0;
+    if (active && lane() == leader) {
+      b0 = bins[bin];
+      bins[bin] = b0 + __popc(peers);
+    }
+    return __shfl_sync(0xffffffffu, b0, leader) + rank(peers);
+  }
+  __device__ __forceinline__ void copyWords(u64* __restrict__ dst, const u64* __restrict__ src, int nw) const {
+    const ulonglong2* s2 = reinterpret_cast<const ulonglong2*>(src);
+    ulonglong2* d2 = reinterpret_cast<ulonglong2*>(dst);
+    const int n2 = nw >> 1;
+    int w = lane();
+    for (; w + 96 < n2; w += 128) {  // 4 independent 16-byte loads in flight per lane
+      ulonglong2 a = s2[w], b = s2[w + 32], c = s2[w + 64], e = s2[w + 96];
+      d2[w] = a;
+      d2[w + 32] = b;
+      d2[w + 64] = c;
+      d2[w + 96] = e;
+    }
+    for (; w < n2; w += 32) d2[w] = s2[w];
+  }
   __device__ __forceinline__ int sum(int v) const { return __reduce_add_sync(0xffffffffu, v); }
   __device__ __forceinline__ int maxv(int v) const { return __reduce_max_sync(0xffffffffu, v); }
   __device__ __forceinline__ int minv(int v) const { return __reduce_min_sync(0xffffffffu, v); }
@@ -356,6 +414,51 @@ WTG_HD int gsfScoreScalarC(const Dev& d, int n, const QEntry& e, int cV, int cI,
   return gsfScoreFrom(l, size, cV, WTG_POPC64(s), (s & v) != 0, WTG_POPC64(i | s), WTG_POPC64(i | s | v), (s & i) != 0);
 }
 
+// this lane's share of |indiv ∪ sig|, |indiv ∪ sig ∪ verified| and of the two intersections, over nw words
+template <class C>
+WTG_HD void poolCounts(C& c, const u64* sig, const u64* rowV, const u64* rowI, int nw, int& cWI, int& cWIV, int& inter, int& interI) {
+  for (int w = c.lane(); w < nw; w += C::LANES) {
+    u64 s = sig[w], v = rowV[w], i = rowI[w];
+    cWI += WTG_POPC64(i | s);
+    cWIV += WTG_POPC64(i | s | v);
+    inter |= (s & v) != 0;
+    interI |= (s & i) != 0;
+  }
+}
+#if defined(__CUDACC__)
+// the warp streams 128-bit loads, four independent triples in flight per lane (nw is even for pooled levels)
+__device__ __forceinline__ void poolCounts(CoopWarp& c, const u64* sig, const u64* rowV, const u64* rowI, int nw, int& cWI, int& cWIV,
+                                           int& inter, int& interI) {
+  const ulonglong2* s2 = reinterpret_cast<const ulonglong2*>(sig);
+  const ulonglong2* v2 = reinterpret_cast<const ulonglong2*>(rowV);
+  const ulonglong2* i2 = reinterpret_cast<const ulonglong2*>(rowI);
+  const int n2 = nw >> 1;
+  for (int w0 = c.lane(); w0 < n2; w0 += 128) {
+    ulonglong2 sv[4], vv[4], iv[4];
+#pragma unroll
+    for (int u = 0; u < 4; ++u) {
+      int w = w0 + 32 * u;
+      if (w < n2) {
+        sv[u] = s2[w];
+        vv[u] = v2[w];
+        iv[u] = i2[w];
+      } else {
+        sv[u] = make_ulonglong2(0, 0);
+        vv[u] = sv[u];
+        iv[u] = sv[u];
+      }
+    }
+#pragma unroll
+    for (int u = 0; u < 4; ++u) {
+      cWI += __popcll(iv[u].x | sv[u].x) + __popcll(iv[u].y | sv[u].y);
+      cWIV += __popcll(iv[u].x | sv[u].x | vv[u].x) + __popcll(iv[u].y | sv[u].y | vv[u].y);
+      inter |= ((sv[u].x & vv[u].x) | (sv[u].y & vv[u].y)) != 0;
+      interI |= ((sv[u].x & iv[u].x) | (sv[u].y & iv[u].y)) != 0;
+    }
+  }
+}
+#endif
+
 // PK_POOL: the whole coop scans the level block
 template <class C>
 WTG_HD int gsfScorePool(const Dev& d, C& c, int n, uint32_t from, uint32_t meta, u64 pl) {
@@ -368,45 +471,7 @@ WTG_HD int gsfScorePool(const Dev& d, C& c, int n, uint32_t from, uint32_t meta,
   const u64* rowI = d.indivVer + (size_t)n * d.W64 + b.w0;
   const u64* sig = d.pool[l] + (size_t)(uint32_t)pl * (size_t)b.nw;
   int cWI = 0, cWIV = 0, inter = 0, interI = 0;
-#if defined(__CUDA_ARCH__)
-  {  // 128-bit loads, four independent triples in flight per lane (nw is even for pooled levels)
-    const ulonglong2* s2 = reinterpret_cast<const ulonglong2*>(sig);
-    const ulonglong2* v2 = reinterpret_cast<const ulonglong2*>(rowV);
-    const ulonglong2* i2 = reinterpret_cast<const ulonglong2*>(rowI);
-    const int n2 = b.nw >> 1;
-    for (int w0 = c.lane(); w0 < n2; w0 += 128) {
-      ulonglong2 sv[4], vv[4], iv[4];
-#pragma unroll
-      for (int u = 0; u < 4; ++u) {
-        int w = w0 + 32 * u;
-        if (w < n2) {
-          sv[u] = s2[w];
-          vv[u] = v2[w];
-          iv[u] = i2[w];
-        } else {
-          sv[u] = make_ulonglong2(0, 0);
-          vv[u] = sv[u];
-          iv[u] = sv[u];
-        }
-      }
-#pragma unroll
-      for (int u = 0; u < 4; ++u) {
-        cWI += __popcll(iv[u].x | sv[u].x) + __popcll(iv[u].y | sv[u].y);
-        cWIV += __popcll(iv[u].x | sv[u].x | vv[u].x) + __popcll(iv[u].y | sv[u].y | vv[u].y);
-        inter |= ((sv[u].x & vv[u].x) | (sv[u].y & vv[u].y)) != 0;
-        interI |= ((sv[u].x & iv[u].x) | (sv[u].y & iv[u].y)) != 0;
-      }
-    }
-  }
-#else
-  for (int w = c.lane(); w < b.nw; w += C::LANES) {
-    u64 s = sig[w], v = rowV[w], i = rowI[w];
-    cWI += WTG_POPC64(i | s);
-    cWIV += WTG_POPC64(i | s | v);
-    inter |= (s & v) != 0;
-    interI |= (s & i) != 0;
-  }
-#endif
+  poolCounts(c, sig, rowV, rowI, b.nw, cWI, cWIV, inter, interI);
   cWI = c.sum(cWI);
   cWIV = c.sum(cWIV);
   bool bi = c.any(inter != 0), bii = c.any(interI != 0);
@@ -499,11 +564,7 @@ WTG_HD void gsfCondScanQueue(const Dev& d, C& c, int n) {
       }
       uint32_t pm = c.ballot(stalePool);
       if (pm) {
-#if defined(__CUDA_ARCH__)
-        int cnt = __popc(pm), off = __popc(pm & ((1u << c.lane()) - 1u));
-#else
-        int cnt = (int)(pm & 1u), off = 0;
-#endif
+        int cnt = c.count(pm), off = c.rank(pm);
         int b0 = 0;
         if (c.lane() == 0) b0 = WTG_ATOMIC_ADD(&d.ctl->workCnt[st], cnt);
         b0 = c.bcast(b0, 0);
@@ -580,11 +641,7 @@ WTG_HD void gsfCondSelect(const Dev& d, C& c, int n, uint32_t* keepBits) {  // n
   for (; base0 < len; base0 += C::LANES) {  // skip the static prefix
     uint32_t kw = keepBits[base0 / C::LANES];
     int inChunk = len - base0 < C::LANES ? len - base0 : C::LANES;
-#if defined(__CUDA_ARCH__)
-    int tot = __popc(kw);
-#else
-    int tot = (int)(kw & 1u);
-#endif
+    int tot = c.count(kw);
     bool hasBest = found && bi >= base0 && bi < base0 + C::LANES;
     if (tot != inChunk || hasBest) break;
     w += tot;
@@ -617,18 +674,13 @@ WTG_HD void gsfCondSelect(const Dev& d, C& c, int n, uint32_t* keepBits) {  // n
       bool keep = false, evict = false;
       uint32_t kw = keepBits[base / C::LANES];
       if (i < len) {
-        bool k0 = (kw >> (C::LANES == 1 ? 0 : c.lane())) & 1u;
+        bool k0 = (kw >> c.lane()) & 1u;
         keep = k0 && !(found && i == bi);
         evict = !k0;
       }
       uint32_t km = c.ballot(keep);
-#if defined(__CUDA_ARCH__)
-      int off = __popc(km & ((1u << c.lane()) - 1u));
-      int tot = __popc(km);
-#else
-      int off = 0;
-      int tot = (int)(km & 1u);
-#endif
+      int off = c.rank(km);
+      int tot = c.count(km);
       if (keep && w + off != i) {
         q[w + off] = e[u];
         qsc[w + off] = es[u];
@@ -641,7 +693,7 @@ WTG_HD void gsfCondSelect(const Dev& d, C& c, int n, uint32_t* keepBits) {  // n
     c.sync();
   }
   if (found) {
-    int srcLane = (C::LANES == 1) ? 0 : (bi % C::LANES);
+    int srcLane = bi % C::LANES;
     best.from = (uint32_t)c.bcast((int)best.from, srcLane);
     best.meta = (uint32_t)c.bcast((int)best.meta, srcLane);
     best.pl = c.bcast64(best.pl, srcLane);
@@ -703,31 +755,18 @@ WTG_HD void gsfLevelCounters(const Dev& d, int n, int l, int& cV, int& cI, int& 
   cU = d.cntUnion[n * d.L + l];
 }
 
-// number of consecutive complete levels: levels 0..k complete (getLastFinishedLevel :193-210)
-WTG_HD int gsfLastFinished(const Dev& d, int n) {
-  int k = 0;
-  for (int j = 1; j < d.L; ++j) {
-    if (d.cntVer[n * d.L + j] == (1 << (j - 1)))
-      k = j;
-    else
-      break;
-  }
-  return k;
-}
+// Per-level scalars of a node are handled "levels as lanes": lane i owns the levels k * LANES + i for k < 32 / LANES
+// (a warp: one level per lane; one lane: every level in turn), and level masks are built from per-round ballots.
 
-// same, with one lane per level: L independent loads instead of a chain of dependent ones
+// number of consecutive complete levels: levels 0..k complete (getLastFinishedLevel :193-210)
 template <class C>
-WTG_HD int gsfLastFinishedCoop(const Dev& d, C& c, int n) {
-  if (C::LANES == 1) return gsfLastFinished(d, n);
-  int l = c.lane();
-  bool complete = l >= 1 && l < d.L && d.cntVer[n * d.L + l] == (1 << (l - 1));
-  uint32_t m = c.ballot(complete);
-  uint32_t t = ~(m >> 1);
-#if defined(__CUDA_ARCH__)
-  return __ffs(t) - 1;
-#else
-  return __builtin_ctz(t);
-#endif
+WTG_HD int gsfLastFinishedLevel(const Dev& d, C& c, int n) {
+  uint32_t comp = 0;
+  for (int k = 0; k < 32 / C::LANES; ++k) {
+    const int l = k * C::LANES + c.lane();
+    comp |= c.ballot(l >= 1 && l < d.L && d.cntVer[n * d.L + l] == (1 << (l - 1))) << (k * C::LANES);
+  }
+  return WTG_CTZ32(~(comp >> 1));
 }
 
 // onNewSig (GSFSignature.java:537-555) — executed by lane 0 only
@@ -927,7 +966,7 @@ WTG_HD void gsfUpdate(const Dev& d, C& c, int n, uint32_t from, uint32_t meta, u
   c.sync();
 
   if (d.accel > 0) {  // :438-451
-    int kf = gsfLastFinishedCoop(d, c, n);
+    int kf = gsfLastFinishedLevel(d, c, n);
     // count the sends first so the descriptor block can be allocated in one go
     int nSend = 0;
     for (int cur = l; cur <= kf && cur < L - 1;) {
@@ -989,239 +1028,105 @@ WTG_HD void gsfUpdate(const Dev& d, C& c, int n, uint32_t from, uint32_t meta, u
 // doCycle  (GSFSignature.java:212-224 + SFLevel.doCycle :313-323) and the periodic re-arm
 // (messages/PeriodicTask.java:40-47)
 // ------------------------------------------------------------------------------------------
+// Levels as lanes: the per-level scalars (cardinality, remainingCalls, cursor, next peer) are loaded and decided by the
+// level's lane; only the payload snapshots are copied by the whole coop.  The send pass reloads what it needs instead of
+// keeping it per level, so the one-lane form holds no per-level arrays.
 template <class C>
-WTG_HD void gsfCycle(const Dev& d, C& c, int n, int item, int& outSlots, int& outDraws) {
+WTG_HD void gsfDoCycle(const Dev& d, C& c, int n, int item, int& outSlots, int& outDraws) {
+  constexpr int K = 32 / C::LANES;
   const int L = d.L;
   const int tick = d.ctl->tick;
   const u64* rowV = d.verified + (size_t)n * d.W64;
-  int kf = gsfLastFinished(d, n);
-  // pass 1: which levels send
+  const int kf = gsfLastFinishedLevel(d, c, n);
   uint32_t sendMask = 0;
-  {
-    int prefix = 1;
-    for (int l = 1; l < L; ++l) {
-      int card = (kf >= l - 1) ? (1 << kf) : prefix;
-      bool started = tick >= l * d.timeoutPerLevel || card >= (1 << (l - 1));  // hasStarted :291-311
-      if (d.remaining[n * L + l] > 0 && started) sendMask |= 1u << l;
-      prefix += d.cntVer[n * L + l];
-    }
+  int carry = 0;
+  for (int k = 0; k < K; ++k) {
+    const int l = k * C::LANES + c.lane();
+    const bool valid = l >= 1 && l < L;
+    const int cv = l < L ? d.cntVer[n * L + l] : 0;
+    const int rem = valid ? d.remaining[n * L + l] : 0;
+    int total;
+    const int prefix = carry + c.exclusiveScan(cv, total);  // sum of the cardinalities of levels 0..l-1
+    carry += total;
+    const int size = valid ? (1 << (l - 1)) : 0;
+    const int card = (kf >= l - 1) ? (1 << kf) : prefix;
+    const bool started = tick >= l * d.timeoutPerLevel || card >= size;  // hasStarted :291-311
+    sendMask |= c.ballot(valid && rem > 0 && started) << (k * C::LANES);
   }
-#if defined(__CUDA_ARCH__)
-  int nSend = __popc(sendMask);
-#else
-  int nSend = __builtin_popcount(sendMask);
-#endif
-  int base = descAlloc(d, c, n, nSend + 1);
-  int sub = 0;
-  long long sentBytes = 0;
+  const int nSend = WTG_POPC32(sendMask);
+  const int base = descAlloc(d, c, n, nSend + 1);
   unsigned long long words = 0;
-  int prefix = 1;
-  for (int l = 1; l < L; ++l) {
-    int cvl = d.cntVer[n * L + l];
-    if (sendMask & (1u << l)) {
-      uint32_t dest = 0;
-      gsfTakePeers(d, c, n, l, 1, &dest);
-      uint32_t meta;
-      u64 pl = 0;
+  int bytes = 0;
+  carry = 0;
+  for (int k = 0; k < K; ++k) {
+    const int l = k * C::LANES + c.lane();
+    const bool snd = (sendMask >> l) & 1u;
+    const int size = l >= 1 && l < L ? (1 << (l - 1)) : 0;
+    int total;
+    const int prefix = carry + c.exclusiveScan(l < L ? d.cntVer[n * L + l] : 0, total);
+    carry += total;
+    uint32_t dest = 0, meta = 0, slot = 0;
+    u64 pl = 0;
+    bool pooled = false;
+    int stagedOn = -1;
+    if (snd) {
+      const int p = d.pos[n * L + l];
+      dest = peerAt(d, n, l, p);  // getRemainingPeers(1) :325-349
+      d.pos[n * L + l] = p + 1 >= size ? 0 : p + 1;
+      d.remaining[n * L + l] -= 1;
       if (kf >= l - 1) {
         meta = metaMake(PK_FULL, (uint32_t)l, (uint32_t)kf);
-      } else {
+      } else if (l <= INLINE_MAX_LEVEL) {
         Blk ob = levelBlock(n, l);  // our own half: what the receiver waits for at its level l
-        if (l <= INLINE_MAX_LEVEL) {
-          meta = metaMake(PK_INLINE, (uint32_t)l, 0);
-          pl = rowV[ob.w0] & ob.mask;
+        meta = metaMake(PK_INLINE, (uint32_t)l, 0);
+        pl = rowV[ob.w0] & ob.mask;
+      } else {
+        meta = metaMake(PK_POOL, (uint32_t)l, 0);
+        const int q = ownerOf(d, (int)dest);
+        if (q != d.rank) {  // the receiver lives on another shard: the snapshot goes into its staging area
+          int off = xStageAlloc(d, q, poolWords(l));
+          pooled = off >= 0;
+          slot = (uint32_t)(pooled ? off : 0);
+          meta |= META_STAGED | ((uint32_t)d.rank << META_SRC_SHIFT);
+          stagedOn = q;
         } else {
-          meta = metaMake(PK_POOL, (uint32_t)l, 0);
-          uint32_t slot = 0;
-          int ok = 1;
-          const int q = ownerOf(d, (int)dest);
-          u64* dst = nullptr;
-          if (q != d.rank) {  // the receiver lives on another shard: the snapshot goes into its staging area
-            int off = 0;
-            if (c.lane() == 0) off = xStageAlloc(d, q, ob.nw);
-            off = c.bcast(off, 0);
-            ok = off >= 0;
-            slot = (uint32_t)(ok ? off : 0);
-            meta |= META_STAGED | ((uint32_t)d.rank << META_SRC_SHIFT);
-            if (ok) dst = xStagePtr(d, q, d.rank, off);
-          } else {
-            if (c.lane() == 0) ok = poolAlloc(d, l, n, slot) ? 1 : 0;
-            slot = (uint32_t)c.bcast((int)slot, 0);
-            ok = c.bcast(ok, 0);
-            if (ok) dst = d.pool[l] + (size_t)slot * (size_t)ob.nw;
-          }
-          if (ok) {
-            for (int w = c.lane(); w < ob.nw; w += C::LANES) dst[w] = rowV[ob.w0 + w];
-            words += (unsigned long long)(2 * ob.nw);
-          }
-          pl = (u64)slot | ((u64)(uint32_t)prefix << 32);
+          pooled = poolAlloc(d, l, n, slot);
         }
+        pl = (u64)slot | ((u64)(uint32_t)prefix << 32);
       }
-      sentBytes += msgSize(l);
-      if (base >= 0 && c.lane() == 0) {
-        Desc ds;
-        ds.dkind = DK_SEND_SINGLE;
-        ds.item = (uint32_t)(d.nLoc + item);
-        ds.sub = (uint32_t)sub;
-        ds.from = (uint32_t)n;
-        ds.to = dest;
-        ds.nDest = 1;
-        ds.evKind = EV_MSG;
-        ds.meta = meta;
-        ds.pl = pl;
-        ds.target = 0;
-        ds.aux = 0;
-        d.desc[base + sub] = ds;
-      }
-      ++sub;
     }
-    prefix += cvl;
-  }
-  if (c.lane() == 0) {
-    if (base >= 0) {  // re-arm: network.sendArriveAt(this, time + period, sender, sender)
+    uint32_t pm = c.ballot(pooled);
+    while (pm) {
+      const int src = c.first(pm);
+      pm &= pm - 1;
+      const int ls = k * C::LANES + src;
+      const uint32_t sl = (uint32_t)c.bcast((int)slot, src);
+      const int so = c.bcast(stagedOn, src);
+      Blk ob = levelBlock(n, ls);
+      u64* dstp = so >= 0 ? xStagePtr(d, so, d.rank, (int)sl) : d.pool[ls] + (size_t)sl * (size_t)ob.nw;
+      c.copyWords(dstp, rowV + ob.w0, ob.nw);
+      words += (unsigned long long)(2 * ob.nw);
+    }
+    if (snd && base >= 0) {
+      const int sub = WTG_POPC32(sendMask & ((1u << l) - 1u));
       Desc ds;
-      ds.dkind = DK_INSERT_AT;
+      ds.dkind = DK_SEND_SINGLE;
       ds.item = (uint32_t)(d.nLoc + item);
       ds.sub = (uint32_t)sub;
       ds.from = (uint32_t)n;
-      ds.to = (uint32_t)n;
-      ds.nDest = 0;
-      ds.evKind = EV_PERIODIC;
-      ds.meta = 0;
-      ds.pl = 0;
-      ds.target = tick + d.period;
+      ds.to = dest;
+      ds.nDest = 1;
+      ds.evKind = EV_MSG;
+      ds.meta = meta;
+      ds.pl = pl;
+      ds.target = 0;
       ds.aux = 0;
       d.desc[base + sub] = ds;
     }
-    d.msgSent[n] += nSend;
-    d.bytesSent[n] += sentBytes;
-    statAdd(d, n, ST_CYCLES, 1ULL);
-    statAdd(d, n, ST_SENDS, (unsigned long long)nSend);
-    if (words) statAdd(d, n, ST_SENDWORDS, words);
+    bytes += snd ? msgSize(l) : 0;
   }
-  c.sync();
-  outSlots = nSend + 1;
-  outDraws = nSend;
-}
-
-#if defined(__CUDACC__)
-// 128-bit lane-strided copy of `nw` 64-bit words (nw even, both sides 16-byte aligned)
-__device__ __forceinline__ void warpCopyWords(u64* __restrict__ dst, const u64* __restrict__ src, int nw, int lane) {
-  const ulonglong2* s2 = reinterpret_cast<const ulonglong2*>(src);
-  ulonglong2* d2 = reinterpret_cast<ulonglong2*>(dst);
-  const int n2 = nw >> 1;
-  int w = lane;
-  for (; w + 96 < n2; w += 128) {  // 4 independent 16-byte loads in flight per lane
-    ulonglong2 a = s2[w], b = s2[w + 32], c = s2[w + 64], e = s2[w + 96];
-    d2[w] = a;
-    d2[w + 32] = b;
-    d2[w + 64] = c;
-    d2[w + 96] = e;
-  }
-  for (; w < n2; w += 32) d2[w] = s2[w];
-}
-
-// doCycle with one lane per level: all per-level scalars (cardinalities, remainingCalls, cursor, next peer) are
-// loaded and decided in parallel; only the payload snapshots are copied cooperatively.  Same results as gsfCycle.
-__device__ __forceinline__ void gsfCycleWarp(const Dev& d, CoopWarp& c, int n, int item, int& outSlots, int& outDraws) {
-  const unsigned FULLM = 0xffffffffu;
-  const int lane = threadIdx.x & 31;
-  const int L = d.L;
-  const int tick = d.ctl->tick;
-  const int l = lane;
-  const bool valid = l >= 1 && l < L;
-  const u64* rowV = d.verified + (size_t)n * d.W64;
-  int cv = l < L ? d.cntVer[n * L + l] : 0;
-  int rem = valid ? d.remaining[n * L + l] : 0;
-  int p = valid ? d.pos[n * L + l] : 0;
-  const int size = valid ? (1 << (l - 1)) : 0;
-  unsigned comp = __ballot_sync(FULLM, valid && cv == size);
-  int kf = __ffs(~(comp >> 1)) - 1;  // levels 1..kf complete (getLastFinishedLevel)
-  int inc = cv;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    int t = __shfl_up_sync(FULLM, inc, o);
-    if (lane >= o) inc += t;
-  }
-  const int prefix = inc - cv;  // sum of the cardinalities of levels 0..l-1
-  const int card = (kf >= l - 1) ? (1 << kf) : prefix;
-  const bool started = tick >= l * d.timeoutPerLevel || card >= size;  // hasStarted :291-311
-  const bool snd = valid && rem > 0 && started;
-  const unsigned sendMask = __ballot_sync(FULLM, snd);
-  const int nSend = __popc(sendMask);
-  int base = 0;
-  if (lane == 0) {
-    int st = n & (ARENA_STRIPES - 1), per = d.descCap / ARENA_STRIPES;
-    int i = atomicAdd(&d.ctl->descCnt[st], nSend + 1);
-    if (i + nSend + 1 > per) {
-      setError(d, ERR_DESC_OVERFLOW, i);
-      base = -1;
-    } else {
-      base = st * per + i;
-    }
-  }
-  base = __shfl_sync(FULLM, base, 0);
-  const int sub = __popc(sendMask & ((1u << lane) - 1u));
-  uint32_t dest = 0, meta = 0, slot = 0;
-  u64 pl = 0;
-  bool pooled = false;
-  int stagedOn = -1;
-  if (snd) {
-    dest = peerAt(d, n, l, p);  // getRemainingPeers(1) :325-349
-    int p2 = p + 1 >= size ? 0 : p + 1;
-    d.pos[n * L + l] = p2;
-    d.remaining[n * L + l] = rem - 1;
-    if (kf >= l - 1) {
-      meta = metaMake(PK_FULL, (uint32_t)l, (uint32_t)kf);
-    } else if (l <= INLINE_MAX_LEVEL) {
-      Blk ob = levelBlock(n, l);
-      meta = metaMake(PK_INLINE, (uint32_t)l, 0);
-      pl = rowV[ob.w0] & ob.mask;
-    } else {
-      meta = metaMake(PK_POOL, (uint32_t)l, 0);
-      const int q = ownerOf(d, (int)dest);
-      if (q != d.rank) {  // the receiver lives on another shard: the snapshot goes into its staging area
-        int off = xStageAlloc(d, q, poolWords(l));
-        pooled = off >= 0;
-        slot = (uint32_t)(pooled ? off : 0);
-        meta |= META_STAGED | ((uint32_t)d.rank << META_SRC_SHIFT);
-        stagedOn = q;
-      } else {
-        pooled = poolAlloc(d, l, n, slot);
-      }
-      pl = (u64)slot | ((u64)(uint32_t)prefix << 32);
-    }
-  }
-  unsigned pm = __ballot_sync(FULLM, pooled);
-  unsigned long long words = 0;
-  while (pm) {
-    int src = __ffs(pm) - 1;
-    pm &= pm - 1;
-    uint32_t sl = __shfl_sync(FULLM, slot, src);
-    int so = __shfl_sync(FULLM, stagedOn, src);
-    Blk ob = levelBlock(n, src);  // our own half of level `src`: what the receiver waits for at its level
-    u64* dstp = so >= 0 ? xStagePtr(d, so, d.rank, (int)sl) : d.pool[src] + (size_t)sl * (size_t)ob.nw;
-    warpCopyWords(dstp, rowV + ob.w0, ob.nw, lane);
-    words += (unsigned long long)(2 * ob.nw);
-  }
-  if (snd && base >= 0) {
-    Desc ds;
-    ds.dkind = DK_SEND_SINGLE;
-    ds.item = (uint32_t)(d.nLoc + item);
-    ds.sub = (uint32_t)sub;
-    ds.from = (uint32_t)n;
-    ds.to = dest;
-    ds.nDest = 1;
-    ds.evKind = EV_MSG;
-    ds.meta = meta;
-    ds.pl = pl;
-    ds.target = 0;
-    ds.aux = 0;
-    d.desc[base + sub] = ds;
-  }
-  int bytes = snd ? msgSize(l) : 0;
-  bytes = __reduce_add_sync(FULLM, bytes);
-  if (lane == 0) {
+  bytes = c.sum(bytes);
+  if (c.lane() == 0) {
     if (base >= 0) {  // re-arm: network.sendArriveAt(this, time + period, sender, sender)
       Desc ds;
       ds.dkind = DK_INSERT_AT;
@@ -1243,11 +1148,10 @@ __device__ __forceinline__ void gsfCycleWarp(const Dev& d, CoopWarp& c, int n, i
     statAdd(d, n, ST_SENDS, (unsigned long long)nSend);
     if (words) statAdd(d, n, ST_SENDWORDS, words);
   }
-  __syncwarp();
+  c.sync();
   outSlots = nSend + 1;
   outDraws = nSend;
 }
-#endif
 
 // ------------------------------------------------------------------------------------------
 // SanFerminSignature handlers (protocols/SanFerminSignature.java, SanFerminHelper.java) — scalar: per-node
@@ -1533,14 +1437,7 @@ WTG_HD void deliver(const Dev& d, C& c, int n, const Ev& ev, uint32_t from, uint
       gsfUpdate(d, c, n, from, meta, pl, item, slots, draws);
     } else {
       if (c.lane() == 0) statAdd(d, n, ST_TASKS, 1ULL);
-#if defined(__CUDA_ARCH__)
-      if constexpr (C::LANES == 32)
-        gsfCycleWarp(d, c, n, item, slots, draws);
-      else
-        gsfCycle(d, c, n, item, slots, draws);
-#else
-      gsfCycle(d, c, n, item, slots, draws);
-#endif
+      gsfDoCycle(d, c, n, item, slots, draws);
     }
   } else if (d.proto == PROTO_CASPER) {
     casperDeliver(d, c, n, ev.kind, meta, pl, item, slots, draws);
@@ -1624,11 +1521,7 @@ WTG_HD int nodeProcess(const Dev& d, C& c, int n, int filter, u64* skippedWord =
     }
     int mn = c.minv(bestItem);
     uint32_t who = c.ballot(bestItem == mn);
-#if defined(__CUDA_ARCH__)
-    int src = __ffs(who) - 1;
-#else
-    int src = __builtin_ctz(who);
-#endif
+    int src = c.first(who);
     u64 w = c.bcast64(bestW, src);
     lastItem = mn;
     int item = inboxItem(w), entry = inboxEntry(w);
@@ -1766,19 +1659,6 @@ WTG_HD int multiUpper(const Dev& d, const MultiRec& rc, int tick) {  // first in
   }
   return lo;
 }
-// rank of this lane among the lanes with `flag` set, and their number (warp ballot; the 1-lane host coop is trivial)
-template <class C>
-WTG_HD int coopRank(C& c, bool flag, int& total) {
-  uint32_t m = c.ballot(flag);
-#if defined(__CUDA_ARCH__)
-  if (C::LANES == 32) {
-    total = __popc(m);
-    return __popc(m & ((1u << c.lane()) - 1u));
-  }
-#endif
-  total = (int)(m & 1u);
-  return 0;
-}
 // first destination index of the group a bucket entry stands for: the record's own cursor, or — replicated sendAll records
 // of a node-sharded run, where every shard walks its own copy — the index carried by the entry
 WTG_HD int multiCur(const Dev& d, const Ev& ev, const MultiRec& rc) { return d.G > 1 ? (int)(uint32_t)ev.pl : (int)rc.cur; }
@@ -1807,9 +1687,7 @@ WTG_HD void dispatchCountCoop(const Dev& d, C& c, int i) {
         int j = j0 + c.lane();
         bool mine = j < up && ownerOf(d, (int)d.recDest[rc.off + j]) == d.rank;
         if (mine) WTG_ATOMIC_ADD(&d.inboxCnt[d.recDest[rc.off + j]], 1);
-        int tot;
-        coopRank(c, mine, tot);
-        m += tot;
+        m += c.count(c.ballot(mine));
       }
       const bool rep = up < (int)rc.n && up > cur && ownerOf(d, (int)d.recDest[rc.off + up - 1]) == d.rank;
       if (c.lane() == 0) d.subCount[p] = m + (rep ? 1 : 0);
@@ -1872,14 +1750,14 @@ WTG_HD void dispatchScatterCoop(const Dev& d, C& c, int i) {
       int j = j0 + c.lane();
       int to = j < up ? (int)d.recDest[rc.off + j] : -1;
       bool mine = j < up && ownerOf(d, to) == d.rank;
-      int tot;
-      int r = coopRank(c, mine, tot);
+      const uint32_t mm = c.ballot(mine);
+      const int r = c.rank(mm);
       if (mine) {
         int s = d.inboxOff[to] + WTG_ATOMIC_ADD(&d.inboxFill[to], 1);
         d.inbox[s] = inboxMake(item0 + m + r, i);
         d.itemKey[item0 + m + r] = bkey | keySub(j);
       }
-      m += tot;
+      m += c.count(mm);
     }
     c.sync();
     if (c.lane() == 0 && up < (int)rc.n && up > cur && ownerOf(d, (int)d.recDest[rc.off + up - 1]) == d.rank) {
