@@ -41,8 +41,10 @@ void wtg_destroy(wtg_net* net);
  * all handles are handed to wtg_shard_link of every shard (same-process shards are mapped directly with peer access,
  * other processes through CUDA IPC), and from then on every shard calls wtg_run_ms with the same arguments.  The data
  * path between shards is device-to-device stores inside the tick kernels (no host call, no collective per tick).
- * Node-indexed read-backs of a shard (counters, GSF rows / scalars) cover its own ids only: wtg_shard_range.
- * Available for GSFSignature; the other protocols refuse to initialise on a sharded network. */
+ * Node-indexed read-backs of a shard (counters, GSF / Handel rows and scalars, CasperIMD node state) cover its own ids
+ * only: wtg_shard_range.  Available for GSFSignature, Handel and CasperIMD; the other protocols refuse to initialise on a
+ * sharded network.  Latency models with multi-second arrivals (no far-future calendar for messages on sharded networks)
+ * and caller-issued sends (wtg_send*) are refused there too. */
 wtg_net* wtg_shard_create(int rank, int world, int device /* -1: default */);
 int wtg_shard_export(wtg_net* net, unsigned char* handle128);
 int wtg_shard_link(wtg_net* net, const unsigned char* handles /* world x 128 bytes, rank order */);
@@ -70,7 +72,9 @@ int wtg_set_node_builder(wtg_net* net, const char* name);
 int wtg_set_msg_discard_time(wtg_net* net, int ms);
 
 /* device capacities (no reference counterpart): "bcap", "qcap", "pool_slots_per_node", "desc_cap",
- * "rec_cap", "ring", "casper_votes", "casper_blocks"; "force_shuffle_serial" (test hook).  Exceeding a capacity makes wtg_run_ms fail loudly; it never drops events. */
+ * "rec_cap", "ring", "casper_votes", "casper_blocks", "stage_words" (node-sharded GSF / Handel: staging area for pooled payloads that
+ * cross shards, 64-bit words per sending shard and pass parity); test hooks "force_shuffle_serial" (SanFermin family: the
+ * serial shuffle path) and "force_pick_serial" (Handel: checkSigs' level draws walked serially, locally and across shards).  Exceeding a capacity makes wtg_run_ms fail loudly; it never drops events. */
 int wtg_set_tunable(wtg_net* net, const char* key, long long value);
 
 /* new PingPong(params).init() — protocols/PingPong.java:52-57, 82-87 */
@@ -192,6 +196,8 @@ int wtg_cappos_node_scalars(wtg_net* net, int* cpl, int* sigs, int* done, int* t
  * rnd.nextInt(i))); runs on the host the code the emit kernel uses; returns the number of values drawn from the stream */
 int wtg_java_shuffle(unsigned long long state, int n, int* inout);
 
+/* Handel read-backs on a node-sharded network: node_scalars, rows and level_scalars cover the shard's own ids (nLoc in place of
+ * N); peers and ranks fail with "node belongs to another shard" for a node of another shard. */
 /* HNode fields — protocols/Handel.java:280-298: 9 int arrays of N: startAt, nodePairingTime, sigsChecked, sigQueueSize,
  * msgFiltered, currWindowSize, addedCycle, totalSigSize(), total length of the toVerifyAgg lists */
 int wtg_handel_node_scalars(wtg_net* net, int* out9N);

@@ -1,0 +1,24 @@
+"""TEST INFRASTRUCTURE — loads the host build of the device logic (tests/emu) with the pass of a node-sharded Handel network
+(tests/emu/wtg_emu_handel_shards.cpp: the pick exchange between the draw scan and the handlers).  Every other network behaves
+as in tests/emu_lib.py.  Never used by the product package."""
+import os
+import subprocess
+
+from tests.emu_lib import EMU_DIR, ROOT
+from wittgenstein_b200 import _lib
+
+_api = None
+
+
+def api():
+    global _api
+    if _api is not None:
+        return _api
+    so = os.path.join(EMU_DIR, "libwtg_emu_handel.so")
+    src = os.path.join(EMU_DIR, "wtg_emu_handel_shards.cpp")
+    csrc = os.path.join(ROOT, "wittgenstein_b200", "csrc")
+    srcs = [src, os.path.join(EMU_DIR, "wtg_emu.cpp")] + [os.path.join(csrc, f) for f in os.listdir(csrc)]
+    if not os.path.exists(so) or any(os.path.getmtime(s) > os.path.getmtime(so) for s in srcs):
+        subprocess.check_call(["g++", "-O2", "-std=c++17", "-fPIC", "-shared", "-ffp-contract=off", "-o", so, src])
+    _api = _lib.Api(so, "wtgemuh_")
+    return _api

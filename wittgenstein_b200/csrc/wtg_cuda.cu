@@ -128,7 +128,7 @@ __global__ void k_hpick_check(Dev d) {
   if (d.ctl->error) return;
   const int blk = blockIdx.x, nBlk = gridDim.x;
   for (int n = d.n0 + blk * blockDim.x + threadIdx.x; n < d.n0 + d.nLoc; n += nBlk * blockDim.x)
-    if (d.hCandK[n] > 0 && hCondPick(d, n, (u64)d.hDrawBase[n], false) > d.condDraws[n]) d.ctl->hReject = 1;
+    if (d.hCandK[n] > 0 && (d.forcePickSerial || hCondPick(d, n, (u64)d.hDrawBase[n], false) > d.condDraws[n])) d.ctl->hReject = 1;
 }
 __global__ void k_hpick_apply(Dev d) {
   if (d.ctl->error) return;
@@ -138,6 +138,33 @@ __global__ void k_hpick_apply(Dev d) {
   } else if (blk == 0 && threadIdx.x == 0) {  // a rejection shifts every later draw: redo the picks in node order
     u64 idx = 0;
     for (int n = d.n0; n < d.n0 + d.nLoc; ++n) idx += (u64)hCondPick(d, n, idx, true);
+  }
+}
+// node-sharded: the pick exchange (wtg_handel.cuh).  Publication: the k of every local pick into every shard's region; a
+// shard in error still publishes its header (which carries the error)
+__global__ void k_hpick_publish(Dev d) {
+  const int blk = blockIdx.x, nBlk = gridDim.x;
+  if (!d.ctl->error)
+    for (int n = d.n0 + blk * blockDim.x + threadIdx.x; n < d.n0 + d.nLoc; n += nBlk * blockDim.x) hPickPublish(d, n);
+  if (blk == 0 && threadIdx.x == 0) hPickPublishHeader(d);
+}
+// after the wait: replay every pick of the shards up to this one on its presumed position
+__global__ void k_hpick_xcheck(Dev d) {
+  if (d.ctl->error) return;
+  const int blk = blockIdx.x, nBlk = gridDim.x;
+  if (blk == 0 && threadIdx.x == 0) hPickHeaders(d);
+  const int upTo = hPicksBelow(d, d.rank + 1);
+  for (int t = blk * blockDim.x + threadIdx.x; t < upTo; t += nBlk * blockDim.x)
+    if (hPickRejects(d, t)) d.ctl->hReject = 1;
+}
+__global__ void k_hpick_xapply(Dev d) {
+  if (d.ctl->error) return;
+  const int blk = blockIdx.x, nBlk = gridDim.x;
+  if (!d.ctl->hReject) {
+    const u64 below = (u64)hPicksBelow(d, d.rank);
+    for (int n = d.n0 + blk * blockDim.x + threadIdx.x; n < d.n0 + d.nLoc; n += nBlk * blockDim.x) hCondPick(d, n, below + (u64)d.hDrawBase[n], true);
+  } else if (blk == 0 && threadIdx.x == 0) {  // a rejection shifts every later draw, on this shard and above
+    hPickSerial(d);
   }
 }
 
@@ -852,11 +879,23 @@ class CudaBackend : public Backend {
         profBegin(P_SCAN_FINAL);
         k_scan_final<<<wide, SCAN_THREADS, 0, st>>>(d, 2);
         profEnd();
-        profBegin(P_COND_SELECT);
-        k_hpick_check<<<sms, 256, 0, st>>>(d);
-        k_hpick_apply<<<sms, 256, 0, st>>>(d);
-        profEnd();
-        launches += 3;
+        if (d.G > 1) {  // node-sharded: the pick exchange puts the picks of the lower shards first
+          profBegin(P_EXCHANGE);
+          k_hpick_publish<<<sms, 256, 0, st>>>(d);
+          k_x_sync<<<1, 32, 0, st>>>(d, 3);
+          profEnd();
+          profBegin(P_COND_SELECT);
+          k_hpick_xcheck<<<sms, 256, 0, st>>>(d);
+          k_hpick_xapply<<<sms, 256, 0, st>>>(d);
+          profEnd();
+          launches += 5;
+        } else {
+          profBegin(P_COND_SELECT);
+          k_hpick_check<<<sms, 256, 0, st>>>(d);
+          k_hpick_apply<<<sms, 256, 0, st>>>(d);
+          profEnd();
+          launches += 3;
+        }
       }
     }
     if (mode != 2 && mode != 3) {  // dispatch and handlers

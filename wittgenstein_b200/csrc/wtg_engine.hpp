@@ -119,11 +119,12 @@ class Engine {
   long long stageWordsWanted = 0;  // protocol-specific staging capacity per (sender, parity), in 64-bit words
   long long farWanted = 0;         // protocol-specific size of the far-future calendar when the latency model needs one
   struct XLayout {
-    size_t hdr, flags, items, newEv, newTarget, stage, rec, recDest, recArrival, beg, all, allCnt, casper, total;
+    size_t hdr, flags, items, newEv, newTarget, stage, rec, recDest, recArrival, beg, all, allCnt, proto, total;
   } xl{};
   // protocol-specific parts of the exchange region, set before allocCommon (CasperIMD: replicated block / attestation tables,
-  // sendAll descriptors of a pass); unevenShards: the protocol's node count need not split into power-of-two shards
-  size_t xCasperBytes = 0;
+  // sendAll descriptors of a pass; Handel: the pick exchange); unevenShards: the protocol's node count need not split into
+  // power-of-two shards
+  size_t xProtoBytes = 0;
   int xAllCapWanted = 0;
   bool unevenShards = false;
   bool shardFarOk = false;  // the protocol's far-future envelopes are tasks of the shard's own nodes
@@ -167,7 +168,7 @@ class Engine {
     q.beg = (XBegin*)(b + xl.beg);
     q.all = (XAll*)(b + xl.all);
     q.allCnt = (int*)(b + xl.allCnt);
-    q.casper = b + xl.casper;
+    q.proto = b + xl.proto;
     return q;
   }
   // exchange region: everything another shard's kernels write (one allocation = one IPC handle)
@@ -175,7 +176,7 @@ class Engine {
     auto al = [](size_t x) { return (x + 255) / 256 * 256; };
     size_t o = 0;
     xl.hdr = o;        o += al(sizeof(XHdr) * MAX_SHARDS);
-    xl.flags = o;      o += al(sizeof(int) * 3 * MAX_SHARDS);
+    xl.flags = o;      o += al(sizeof(int) * 4 * MAX_SHARDS);
     xl.items = o;      o += al(sizeof(XItem) * (size_t)d.G * d.xItemCap);
     xl.newEv = o;      o += al(sizeof(Ev) * (size_t)d.newEvCap);
     xl.newTarget = o;  o += al(sizeof(int) * (size_t)d.newEvCap);
@@ -186,7 +187,7 @@ class Engine {
     xl.beg = o;        o += al(sizeof(XBegin) * MAX_SHARDS);
     xl.all = o;        o += al(sizeof(XAll) * (size_t)d.G * (size_t)std::max(1, d.xAllCap));
     xl.allCnt = o;     o += al(sizeof(int) * MAX_SHARDS);
-    xl.casper = o;     o += al(xCasperBytes);
+    xl.proto = o;      o += al(xProtoBytes);
     xl.total = o;
     xBytes = o;
     xRegion = be->allocShared(o);
@@ -394,6 +395,7 @@ class Engine {
   int recDestOverride = 0;  // sendAll protocols size the destination arena themselves
   int destScratchOverride = 0;
   bool forceShufSerial = false;  // tunable force_shuffle_serial (test hook)
+  bool forcePickSerial = false;  // tunable force_pick_serial (test hook, Handel)
   int ringExtra = 0;        // longest handler-chosen delay of a near envelope (e.g. blockConstructionTime)
   bool farEnabled = false;  // far-future calendar (+ fast-forward for protocols without conditional tasks)
   bool farTicking = false;  // calendar without fast-forward: the latency model, not the protocol, asked for it
@@ -774,11 +776,11 @@ class Engine {
 
   // ---- Handel.init()  (protocols/Handel.java:957-1014).  Everything init() draws from network.rd is sequential
   //      (bad nodes, start times, node attributes, N cumulative shuffles for the reception ranks, tie shuffles of
-  //      the emission lists), so it runs on the host like in the reference; the tables are then uploaded. ----
+  //      the emission lists), so it runs on the host like in the reference; the tables are then uploaded.  Node-sharded:
+  //      every shard runs the whole init (so `rd` ends in the same state everywhere) and keeps its own nodes' state. ----
   HandelParams hp{};
   void handelInit(const HandelParams& p) {
     requireNotInited();
-    requireUnsharded("this protocol");
     const int N = p.nodeCount;
     if (p.nodesDown >= N || p.nodesDown < 0 || p.threshold > N || (p.nodesDown + p.threshold > N))  // :112-117
       throw std::invalid_argument("nodeCount=" + std::to_string(N) + ", threshold=" + std::to_string(p.threshold));
@@ -805,9 +807,22 @@ class Engine {
     }
     int L = 1;
     while ((1 << L) <= N) ++L;
+    if (sharded()) {
+      // pooled payloads that cross shards are staged on the receiving shard (one area per sender and pass parity).  A node
+      // disseminates at most once per pass, one message per level, and only the levels whose sibling block spans whole
+      // shards cross: at most one block of each of those levels per sending node (DESIGN.md §8)
+      const long long nl = N / shardWorld;
+      long long words = 0;
+      for (int l = INLINE_MAX_LEVEL + 1; l < L; ++l)
+        if ((1LL << (l - 1)) >= nl) words += (1LL << (l - 1)) / 64;
+      stageWordsWanted = std::max<long long>(65536, nl * words + 8192);
+      if (tun.stageWords) stageWordsWanted = tun.stageWords;
+      xProtoBytes = hPickBytes(shardWorld, (int)nl);  // the pick exchange: one byte per pick, at most one per node and pass
+    }
     allocCommon(N, PROTO_HANDEL);
     for (int i = 0; i < N; ++i)
       if (startAt[(size_t)i] + 1 >= d.ring) throw std::invalid_argument("desynchronizedStart exceeds the time ring");
+    const int NL = d.nLoc, n0 = d.n0;
     d.L = L;
     d.W64 = std::max(1, N / 64);
     d.threshold = p.threshold;
@@ -821,62 +836,66 @@ class Engine {
     d.hWinMax = 128;
     d.qcap = (int)(tun.qcap ? tun.qcap : std::min<long long>(4096, std::max<long long>(64, 2LL * N)));
     d.qcap = (d.qcap + 31) / 32 * 32;
-    size_t rowWords = (size_t)N * d.W64;
+    const size_t W = (size_t)d.W64;
     // level 0: own signature in lastAggVerified / verifiedIndSignatures / totalIncoming (:409-417); initLevel() runs for every node
-    std::vector<unsigned long long> diag(rowWords, 0);
-    for (int i = 0; i < N; ++i) diag[(size_t)i * d.W64 + (size_t)(i >> 6)] = 1ULL << (i & 63);
-    d.hLastAgg = dupload(diag);
-    d.hTotInc = dupload(diag);
-    d.hVerInd = dupload(diag);
-    d.hToVerInd = dalloc<unsigned long long>(rowWords);
-    d.hFinPeers = dalloc<unsigned long long>(rowWords);
-    d.hBlack = dalloc<unsigned long long>(rowWords);
+    {
+      std::vector<unsigned long long> diag((size_t)NL * W, 0);
+      for (int i = n0; i < n0 + NL; ++i) diag[(size_t)(i - n0) * W + (size_t)(i >> 6)] = 1ULL << (i & 63);
+      for (unsigned long long** row : {&d.hLastAgg, &d.hTotInc, &d.hVerInd}) {
+        *row = dallocNodes<unsigned long long>(W);
+        be->upload(*row + (size_t)n0 * W, diag.data(), diag.size() * sizeof(unsigned long long));
+      }
+    }
+    d.hToVerInd = dallocNodes<unsigned long long>(W);
+    d.hFinPeers = dallocNodes<unsigned long long>(W);
+    d.hBlack = dallocNodes<unsigned long long>(W);
     std::vector<int> zerosNL((size_t)N * L, 0), outFin((size_t)N * L, 0), biz((size_t)N * L, p.byzantineSuicide ? 0 : -1), cnt0((size_t)N * L, 0);
     std::vector<uint32_t> ver((size_t)N * L, 1);
     for (int i = 0; i < N; ++i) {
       outFin[(size_t)i * L] = 1;  // level 0: outgoingFinished = true
       cnt0[(size_t)i * L] = 1;
     }
-    d.hPos = dupload(zerosNL);
-    d.hOutFin = dupload(outFin);
-    d.hBiz = dupload(biz);
+    d.hPos = duploadNodes(zerosNL, L);
+    d.hOutFin = duploadNodes(outFin, L);
+    d.hBiz = duploadNodes(biz, L);
     {
       std::vector<int> nohit((size_t)N * L, -2147483647 - 1);
-      d.hBizNoHit = dupload(nohit);
+      d.hBizNoHit = duploadNodes(nohit, L);
     }
-    d.hCntLast = dupload(cnt0);
-    d.hCntInc = dupload(cnt0);
-    d.hCntInd = dupload(cnt0);
-    d.lvVer = dupload(ver);
+    d.hCntLast = duploadNodes(cnt0, L);
+    d.hCntInc = duploadNodes(cnt0, L);
+    d.hCntInd = duploadNodes(cnt0, L);
+    d.lvVer = duploadNodes(ver, L);
     std::vector<int> ones((size_t)N, 1), win((size_t)N, d.hWinInit), added((size_t)N, p.extraCycle), pairing((size_t)N), minStart((size_t)N);
     for (int i = 0; i < N; ++i) {
       pairing[(size_t)i] = (int)std::max(1.0, p.pairingTime * hm.nodes[(size_t)i].speed);  // :282
       minStart[(size_t)i] = startAt[(size_t)i] + 1;                                        // :981-982
     }
-    d.hTotal = dupload(ones);
-    d.hWindow = dupload(win);
-    d.hAddedCycle = dupload(added);
-    d.pairing = dupload(pairing);
-    d.minStart = dupload(minStart);
-    d.stamp = dalloc<uint32_t>(N);
-    d.hStartAt = dupload(startAt);
-    d.hSigsChecked = dalloc<int>(N);
-    d.hSigQueueSize = dalloc<int>(N);
-    d.hMsgFiltered = dalloc<int>(N);
-    d.hSeq = dalloc<int>(N);
-    d.qLen = dalloc<int>(N);
-    d.hQueue = dalloc<HQEntry>((size_t)N * d.qcap);
-    d.qStamp = dalloc<uint32_t>((size_t)N * d.qcap);
-    d.hCand = dalloc<int>((size_t)N * 32);
-    d.hCandK = dalloc<int>(N);
-    d.hDrawBase = dalloc<int>(N);
+    d.hTotal = duploadNodes(ones);
+    d.hWindow = duploadNodes(win);
+    d.hAddedCycle = duploadNodes(added);
+    d.pairing = duploadNodes(pairing);
+    d.minStart = duploadNodes(minStart);
+    d.stamp = dallocNodes<uint32_t>();
+    d.hStartAt = duploadNodes(startAt);
+    d.hSigsChecked = dallocNodes<int>();
+    d.hSigQueueSize = dallocNodes<int>();
+    d.hMsgFiltered = dallocNodes<int>();
+    d.hSeq = dallocNodes<int>();
+    d.qLen = dallocNodes<int>();
+    d.hQueue = dallocNodes<HQEntry>((size_t)d.qcap);
+    d.qStamp = dallocNodes<uint32_t>((size_t)d.qcap);
+    d.hCand = dallocNodes<int>(32);
+    d.hCandK = dallocNodes<int>();
+    d.hDrawBase = dallocNodes<int>();
     d.hHidden = p.hiddenByzantine ? 1 : 0;
-    d.hbNoPeers = dalloc<int>(N);
+    d.forcePickSerial = forcePickSerial ? 1 : 0;
+    d.hbNoPeers = dallocNodes<int>();
     {
       std::vector<int> m1((size_t)N, -1);
-      d.hbLastId = dupload(m1);
+      d.hbLastId = duploadNodes(m1);
     }
-    d.hbLastFrom = dalloc<int>(N);
+    d.hbLastFrom = dallocNodes<int>();
     const bool timing_ = std::getenv("WTG_INIT_TIMING") != nullptr;
     auto t0_ = std::chrono::steady_clock::now();
     auto lap_ = [&](const char* what) {
@@ -886,95 +905,119 @@ class Engine {
       t0_ = t1;
     };
     lap_("nodes + rows");
-    // setReceivingRanks (:940-948): N cumulative shuffles of one list
-    std::vector<int> ranks((size_t)N * N);
+    unsigned hw = std::thread::hardware_concurrency();
+    int T = (int)std::max(1u, std::min(hw ? hw : 1u, 64u));
+    if (N < 2048) T = 1;
+    auto parallelFor = [&](int n, const std::function<void(int, int)>& body) {  // body(begin, end), contiguous chunks
+      if (T == 1) {
+        body(0, n);
+        return;
+      }
+      std::vector<std::thread> th;
+      int per = (n + T - 1) / T;
+      for (int t = 0; t < T; ++t) {
+        int b0 = t * per, b1 = std::min(n, b0 + per);
+        if (b0 < b1) th.emplace_back(body, b0, b1);
+      }
+      for (auto& x : th) x.join();
+    };
+    // setReceivingRanks (:940-948): N cumulative shuffles of one list.  Every shard draws all of them and keeps its own rows
+    // plus the transposed table (the emission list of sender s reads column s, and every sender's tie shuffles draw from rd).
+    // Host peak: the transposed table (N^2) + the own rows (nLoc x N) + the own senders' lists (nLoc x (N-1)).
+    std::vector<int> ranksOwn((size_t)NL * N);
+    std::unique_ptr<int[]> ranksT_(new int[(size_t)N * N]);  // first touched by the transposing threads
+    int* const ranksT = ranksT_.get();
     {
       std::vector<int> expected((size_t)N);
       for (int i = 0; i < N; ++i) expected[(size_t)i] = i;
-      for (int n = 0; n < N; ++n) {
-        for (int i = N; i > 1; --i) std::swap(expected[(size_t)i - 1], expected[(size_t)hm.rd.nextInt(i)]);
-        int* row = ranks.data() + (size_t)n * N;
-        for (int i = 0; i < N; ++i) row[expected[(size_t)i]] = i;
+      const int RB = std::min(N, 1024);  // rows drawn before they are transposed
+      std::vector<int> blk((size_t)RB * N);
+      for (int r0 = 0; r0 < N; r0 += RB) {
+        const int r1 = std::min(N, r0 + RB);
+        for (int n = r0; n < r1; ++n) {
+          for (int i = N; i > 1; --i) std::swap(expected[(size_t)i - 1], expected[(size_t)hm.rd.nextInt(i)]);
+          int* row = blk.data() + (size_t)(n - r0) * N;
+          for (int i = 0; i < N; ++i) row[expected[(size_t)i]] = i;
+        }
+        for (int n = std::max(r0, n0); n < std::min(r1, n0 + NL); ++n)
+          std::memcpy(ranksOwn.data() + (size_t)(n - n0) * N, blk.data() + (size_t)(n - r0) * N, sizeof(int) * (size_t)N);
+        parallelFor(N, [&](int c0, int c1) {  // contiguous writes: rows [r0, r1) of columns [c0, c1)
+          for (int c = c0; c < c1; ++c) {
+            int* dst = ranksT + (size_t)c * N + r0;
+            for (int r = r0; r < r1; ++r) dst[r - r0] = blk[(size_t)(r - r0) * N + c];
+          }
+        });
       }
     }
     lap_("reception ranks");
-    // emission lists (:991-1013): receivers of each level sorted by the rank they gave the sender, ties shuffled
-    std::vector<uint32_t> peers((size_t)N * (size_t)(N - 1), 0);
+    // emission lists (:991-1013): receivers of each level sorted by the rank they gave the sender, ties shuffled.  The order of
+    // every list is a pure function of the rank table; only the shuffles of equal-rank runs draw from the network RNG, and they
+    // must do so in (sender, level, position) order.  Senders go in chunks: their lists are sorted on all host threads (the
+    // lists of the shard's own senders are kept, of the others only the equal-rank runs), then one sequential pass shuffles the
+    // ties of the chunk.
+    std::vector<uint32_t> peersOwn((size_t)NL * (size_t)(N - 1), 0);
     {
-      // The order of every list is a pure function of the rank table; only the shuffles of equal-rank runs draw from the
-      // network RNG, and they must do so in (sender, level, position) order.  So: (1) transpose the table once (the list
-      // of sender s reads column s); (2) sort all lists on all host threads; (3) one sequential pass shuffles the ties.
-      std::unique_ptr<int[]> ranksT_(new int[(size_t)N * N]);  // first touched by the transposing threads
-      int* const ranksT = ranksT_.get();
-      const int TB = 64;
-      auto transposeRows = [&](int r0, int r1) {
-        for (int rb = r0; rb < r1; rb += TB)
-          for (int cb = 0; cb < N; cb += TB)
-            for (int c = cb; c < std::min(cb + TB, N); ++c)  // contiguous writes (15x faster than contiguous reads here)
-              for (int r = rb; r < std::min(rb + TB, r1); ++r) ranksT[(size_t)c * N + r] = ranks[(size_t)r * N + c];
+      struct Run {
+        uint32_t off, len;  // position in the sender's list (all levels), length >= 2
       };
-      auto sortSender = [&](int sIdx, std::vector<unsigned long long>& keys) {
+      const int CH = std::min(N, 16 * T);
+      std::vector<std::vector<Run>> runs((size_t)CH);
+      auto ownList = [&](int sIdx) { return sIdx >= n0 && sIdx < n0 + NL ? peersOwn.data() + (size_t)(sIdx - n0) * (size_t)(N - 1) : nullptr; };
+      auto sortSender = [&](int sIdx, std::vector<unsigned long long>& keys, std::vector<Run>& rs) {
+        rs.clear();
         if (hm.nodes[(size_t)sIdx].down) return;
         const int* col = ranksT + (size_t)sIdx * N;
+        uint32_t* list = ownList(sIdx);
         for (int l = 1; l < L; ++l) {
           Blk wb = levelBlock(sIdx ^ (1 << (l - 1)), l);
           keys.resize((size_t)wb.size);
           for (int i = 0; i < wb.size; ++i)  // unique keys: (rank, receiver) — ascending receiver inside a tie == stable order
             keys[(size_t)i] = ((unsigned long long)(uint32_t)col[wb.base + i] << 32) | (unsigned long long)(uint32_t)(wb.base + i);
           std::sort(keys.begin(), keys.end());
-          uint32_t* out = peers.data() + (size_t)sIdx * (size_t)(N - 1) + (size_t)((1 << (l - 1)) - 1);
-          for (int i = 0; i < wb.size; ++i) out[i] = (uint32_t)(keys[(size_t)i] & 0xFFFFFFFFULL);
-        }
-      };
-      unsigned hw = std::thread::hardware_concurrency();
-      int T = (int)std::max(1u, std::min(hw ? hw : 1u, 64u));
-      if (N < 2048) T = 1;
-      auto parallelFor = [&](int n, const std::function<void(int, int)>& body) {  // body(begin, end), contiguous chunks
-        if (T == 1) {
-          body(0, n);
-          return;
-        }
-        std::vector<std::thread> th;
-        int per = (n + T - 1) / T;
-        for (int t = 0; t < T; ++t) {
-          int b0 = t * per, b1 = std::min(n, b0 + per);
-          if (b0 < b1) th.emplace_back(body, b0, b1);
-        }
-        for (auto& x : th) x.join();
-      };
-      parallelFor(N, [&](int r0, int r1) { transposeRows(r0, r1); });
-      lap_("rank table transpose");
-      parallelFor(N, [&](int s0, int s1) {
-        std::vector<unsigned long long> keys;
-        for (int sIdx = s0; sIdx < s1; ++sIdx) sortSender(sIdx, keys);
-      });
-      lap_("emission lists: sort");
-      for (int sIdx = 0; sIdx < N; ++sIdx) {  // Collections.shuffle of every run of equal ranks, in the reference's order
-        if (hm.nodes[(size_t)sIdx].down) continue;
-        const int* col = ranksT + (size_t)sIdx * N;
-        for (int l = 1; l < L; ++l) {
-          const int size = 1 << (l - 1);
-          uint32_t* out = peers.data() + (size_t)sIdx * (size_t)(N - 1) + (size_t)(size - 1);
-          for (int i = 0; i < size;) {
+          const uint32_t lo = (1u << (l - 1)) - 1u;
+          if (list)
+            for (int i = 0; i < wb.size; ++i) list[lo + (uint32_t)i] = (uint32_t)(keys[(size_t)i] & 0xFFFFFFFFULL);
+          for (int i = 0; i < wb.size;) {
             int j = i + 1;
-            const int rk = col[out[i]];
-            while (j < size && col[out[j]] == rk) ++j;
-            for (int m = j - i; m > 1; --m) std::swap(out[i + m - 1], out[i + hm.rd.nextInt(m)]);
+            while (j < wb.size && (keys[(size_t)j] >> 32) == (keys[(size_t)i] >> 32)) ++j;
+            if (j - i > 1) rs.push_back(Run{lo + (uint32_t)i, (uint32_t)(j - i)});
             i = j;
           }
+        }
+      };
+      for (int c0 = 0; c0 < N; c0 += CH) {
+        const int c1 = std::min(N, c0 + CH);
+        parallelFor(c1 - c0, [&](int a, int b) {
+          std::vector<unsigned long long> keys;
+          for (int i = a; i < b; ++i) sortSender(c0 + i, keys, runs[(size_t)i]);
+        });
+        for (int sIdx = c0; sIdx < c1; ++sIdx) {  // Collections.shuffle of every run of equal ranks, in the reference's order
+          uint32_t* list = ownList(sIdx);
+          for (const Run& r : runs[(size_t)(sIdx - c0)])
+            for (int m = (int)r.len; m > 1; --m) {
+              const int j = hm.rd.nextInt(m);
+              if (list) std::swap(list[r.off + (uint32_t)m - 1], list[r.off + (uint32_t)j]);
+            }
         }
       }
     }
     lap_("emission lists");
-    d.hRanks = dupload(ranks);
+    ranksT_.reset();
+    {
+      int* pr = dalloc<int>((size_t)NL * N);
+      be->upload(pr, ranksOwn.data(), ranksOwn.size() * sizeof(int));
+      d.hRanks = pr - (size_t)n0 * N;
+      uint32_t* pp = dalloc<uint32_t>((size_t)NL * (size_t)(N - 1));
+      be->upload(pp, peersOwn.data(), peersOwn.size() * sizeof(uint32_t));
+      d.peers = pp - (size_t)n0 * (size_t)(N - 1);
+    }
     d.peerBits = 32;
-    d.peers = dupload(peers);
     lap_("upload");
     Ctl c;
     std::memset(&c, 0, sizeof(c));
     long long perNode = tun.poolSlotsPerNode ? tun.poolSlotsPerNode : 24;
     for (int l = INLINE_MAX_LEVEL + 1; l < L; ++l) {
-      long long slots = std::max<long long>(1024, perNode * N);
+      long long slots = std::max<long long>(1024, perNode * NL);
       slots = (slots + POOL_STRIPES - 1) / POOL_STRIPES * POOL_STRIPES;
       d.poolCap[l] = (int)slots;
       d.pool[l] = dalloc<unsigned long long>((size_t)slots * (size_t)poolWords(l));
@@ -988,9 +1031,11 @@ class Engine {
       d.poolFree[l] = dupload(fl);
       c.poolMinFree[l] = (int)slots;
     }
-    // periodic dissemination at startAt + 1 for live nodes, in id order (:978-983)
+    // periodic dissemination at startAt + 1 for live nodes, in id order (:978-983); a shard registers its own nodes' tasks,
+    // with the ordering key of "pass 0" (wtg_shard.cuh)
     std::vector<std::vector<Ev>> per((size_t)d.ring);
-    for (int i = 0; i < N; ++i)
+    std::vector<std::vector<unsigned long long>> perKey((size_t)d.ring);
+    for (int i = n0; i < n0 + NL; ++i)
       if (!hm.nodes[(size_t)i].down) {
         Ev ev;
         std::memset(&ev, 0, sizeof(ev));
@@ -999,11 +1044,13 @@ class Engine {
         ev.to = (uint32_t)i;
         ev.from = (uint32_t)i;
         per[(size_t)(startAt[(size_t)i] + 1)].push_back(ev);
+        perKey[(size_t)(startAt[(size_t)i] + 1)].push_back(orderKey(0, (unsigned)i));
       }
     for (int t = 0; t < d.ring; ++t)
       if (!per[(size_t)t].empty()) {
         if ((int)per[(size_t)t].size() > d.bcap) throw std::runtime_error("bucket capacity too small");
         be->upload(d.buckets + (size_t)t * d.bcap, per[(size_t)t].data(), per[(size_t)t].size() * sizeof(Ev));
+        if (sharded()) be->upload(d.bucketKey + (size_t)t * d.bcap, perKey[(size_t)t].data(), perKey[(size_t)t].size() * sizeof(unsigned long long));
         int cnt = (int)per[(size_t)t].size();
         be->upload(d.bucketCount + t, &cnt, sizeof(int));
       }
@@ -1115,7 +1162,7 @@ class Engine {
                       // attestation tables are replicated inside the exchange region; periodic tasks are the only far envelopes
       unevenShards = true;
       shardFarOk = true;
-      xCasperBytes = casperTabsBytes((int)maxBlocks, maxAtts, maxAtts / 64);
+      xProtoBytes = casperTabsBytes((int)maxBlocks, maxAtts, maxAtts / 64);
       xAllCapWanted = N / shardWorld + 64;
     }
     allocCommon(N, PROTO_CASPER);
@@ -1150,9 +1197,9 @@ class Engine {
     g.nBlocks = 1;
     g.byzToSend = 1;
     if (sharded()) {
-      std::vector<char> zero(xCasperBytes, 0);
-      be->upload(d.peer[d.rank].casper, zero.data(), zero.size());
-      CasperTabs t = casperTabsAt(d.peer[d.rank].casper, d.cMaxBlocks, d.cMaxAtts);
+      std::vector<char> zero(xProtoBytes, 0);
+      be->upload(d.peer[d.rank].proto, zero.data(), zero.size());
+      CasperTabs t = casperTabsAt(d.peer[d.rank].proto, d.cMaxBlocks, d.cMaxAtts);
       d.cg = t.cg;
       d.cbHeight = t.cbHeight;
       d.cbParent = t.cbParent;
@@ -1421,10 +1468,10 @@ class Engine {
     throw std::runtime_error(std::string("device engine error: ") + names[c.error < 13 ? c.error : 8] + " (detail " + std::to_string(c.errorDetail) + ")");
   }
 
-  // node-sharded sendAll protocols: a multi-destination envelope has one bucket entry on every shard that owns a destination
-  // of its next group; msgs.size() counts it once — on the shard that owns the group's first destination
+  // node-sharded runs: a multi-destination envelope has one bucket entry on every shard that owns a destination of its next
+  // group; msgs.size() counts it once — on the shard that owns the group's first destination
   int countBucket(int slot, int cnt) {
-    if (!(sharded() && d.allCap > 0)) return cnt;
+    if (!sharded()) return cnt;
     std::vector<Ev> evs((size_t)cnt);
     be->download(evs.data(), d.buckets + (size_t)slot * (size_t)d.bcap, evs.size() * sizeof(Ev));
     int c = 0;
@@ -1435,8 +1482,8 @@ class Engine {
       }
       MultiRec rc;
       be->download(&rc, d.rec + e.aux, sizeof(MultiRec));
-      uint32_t first = 0;
-      be->download(&first, d.recDest + rc.off + (uint32_t)e.pl, sizeof(uint32_t));
+      uint32_t first = 0;  // replicated records: the group starts at Ev.pl; shipped record copies: at their cursor
+      be->download(&first, d.recDest + rc.off + (d.allCap > 0 ? (uint32_t)e.pl : rc.cur), sizeof(uint32_t));
       if (ownerOf(d, (int)first) == d.rank) ++c;
     }
     return c;
@@ -1572,8 +1619,8 @@ class Engine {
     be->sync();
     be->upload(d.ndown + id, &v, 1);
     if (d.proto == PROTO_HANDEL) {  // the cached per-level minimum rank of the down peers is stale now
-      std::vector<int> dirty((size_t)d.N * d.L, -2147483647 - 1);
-      be->upload(d.hBizNoHit, dirty.data(), dirty.size() * sizeof(int));
+      std::vector<int> dirty((size_t)d.nLoc * d.L, -2147483647 - 1);
+      be->upload(d.hBizNoHit + (size_t)d.n0 * d.L, dirty.data(), dirty.size() * sizeof(int));
     }
   }
   void uploadPartitions() {

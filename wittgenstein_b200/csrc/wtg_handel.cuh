@@ -9,7 +9,9 @@
 // finishedPeers, blacklist); level l of a node is the aligned block of the row, exactly as for GSF.
 // totalOutgoing(l) is not stored: it always equals the totalIncoming row restricted to the node's own half of
 // level l (it is refreshed from the lower levels' totalIncoming at every improving update, :733-745).
-// HiddenByzantine (:840-917) is not built; the engine rejects the parameter.
+// HiddenByzantine (:840-917) runs inside the pick (hHiddenAttack).
+// Node-sharded runs: pooled payloads for a receiver on another shard are staged on that shard at emission (hStageAtEmit),
+// and the picks' draw indices are made global by the pick exchange (hPick*, after the local draw scan).
 #pragma once
 
 namespace wtg {
@@ -922,24 +924,29 @@ WTG_HD int hHiddenAttack(const Dev& d, int n, int ci) {
   return nb;
 }
 
+// java.util.Random.nextInt(k) at stream index `drawIdx` after ctl.rng: the value in r, the stream values consumed returned
+WTG_HD int hNextInt(const Dev& d, u64 drawIdx, int k, int& r) {
+  int used = 0;
+  for (;;) {
+    u64 st = lcgAdvance(d.jumpA, d.jumpC, d.ctl->rng, drawIdx + (u64)used + 1);
+    ++used;
+    int32_t u = (int32_t)(uint32_t)(st >> 17);
+    if ((k & (k - 1)) == 0) {
+      r = (int)(((long long)k * (long long)u) >> 31);
+      return used;
+    }
+    r = u % k;
+    if ((int32_t)((uint32_t)u - (uint32_t)r + (uint32_t)(k - 1)) >= 0) return used;
+  }
+}
 // phase D: pick the level with network.rd.nextInt(k) and finish checkSigs (:808-837).  `drawIdx` = index of this
 // node's draw in the stream after ctl.rng (exclusive scan of condDraws over nodes).  Returns the number of
 // stream values consumed (1, or more when nextInt's rejection loop fires).
 WTG_HD int hCondPick(const Dev& d, int n, u64 drawIdx, bool apply) {
   int k = d.hCandK[n];
   if (k <= 0) return 0;
-  int used = 0, r;
-  for (;;) {  // java.util.Random.nextInt(bound)
-    u64 st = lcgAdvance(d.jumpA, d.jumpC, d.ctl->rng, drawIdx + (u64)used + 1);
-    ++used;
-    int32_t u = (int32_t)(uint32_t)(st >> 17);
-    if ((k & (k - 1)) == 0) {
-      r = (int)(((long long)k * (long long)u) >> 31);
-      break;
-    }
-    r = u % k;
-    if ((int32_t)((uint32_t)u - (uint32_t)r + (uint32_t)(k - 1)) >= 0) break;
-  }
+  int r;
+  const int used = hNextInt(d, drawIdx, k, r);
   if (!apply) return used;
   int lvl = -1, seen = 0;
   for (int l = 1; l < d.L; ++l)
@@ -984,6 +991,84 @@ WTG_HD int hCondPick(const Dev& d, int n, u64 drawIdx, bool apply) {
   d.condFired[n] = 1;
   d.condDraws[n] = used;
   return used;
+}
+
+// node-sharded runs: a pooled dissemination payload (hMakePayload) whose receiver lives on another shard moves at emission
+// from its slab into that shard's staging area (the slab held only the envelope's reference); k_x2_ingest puts it into a
+// slab there.  Emission never allocates, so the slab goes straight back to its free stack.
+WTG_HD void hStageAtEmit(const Dev& d, Ev& ev) {
+  const int l = (int)metaLevel(ev.meta), nw = poolWords(l), q = ownerOf(d, (int)ev.to);
+  const uint32_t slot = (uint32_t)ev.pl;
+  const int off = xStageAlloc(d, q, nw);
+  if (off >= 0) {
+    const u64* src = d.pool[l] + (size_t)slot * (size_t)nw;
+    u64* dst = xStagePtr(d, q, d.rank, off);
+    for (int w = 0; w < nw; ++w) dst[w] = src[w];
+  }
+  freeDirect(d, l, slot);
+  ev.meta |= META_STAGED | ((uint32_t)d.rank << META_SRC_SHIFT);
+  ev.pl = (ev.pl & 0xFFFFFFFF00000000ULL) | (u64)(uint32_t)(off >= 0 ? off : 0);
+}
+
+// ---- node-sharded runs: the pick exchange ---------------------------------------------------------------------------
+// The conditional pass runs in node-id order before any message of the millisecond, so the level draw of node n sits at
+// (picks of the shards below) + (local exclusive scan of the draws, hDrawBase[n]).  Every pick presumes one draw.  Each shard
+// publishes its sequence of k values (one byte per pick, node order) and its pick count to every shard, then signals; after
+// the wait every shard replays the picks of the pass up to its own on their presumed positions.  None rejects (the common
+// case): the presumed positions are the real ones.  One rejects: one thread walks all picks in order (the first rejection
+// is found at its real position, every later one is shifted), exactly like the unsharded serial path.
+// the pick exchange's part of a shard's exchange region: XPick [G] (256 bytes), then the k values [G][perShard]
+WTG_HD size_t hPickBytes(int G, int perShard) { return 256 + (size_t)G * (size_t)perShard; }
+WTG_HD XPick* hPickHdr(const Dev& d, int q) { return reinterpret_cast<XPick*>(d.peer[q].proto); }
+WTG_HD unsigned char* hPickK(const Dev& d, int q) { return reinterpret_cast<unsigned char*>(d.peer[q].proto) + 256; }
+WTG_HD void hPickPublish(const Dev& d, int n) {
+  const int k = d.hCandK[n];
+  if (k <= 0) return;
+  const size_t at = (size_t)d.rank * (size_t)d.perShard + (size_t)d.hDrawBase[n];
+  for (int q = 0; q < d.G; ++q) hPickK(d, q)[at] = (unsigned char)k;
+}
+WTG_HD void hPickPublishHeader(const Dev& d) {
+  XPick h;
+  h.seq = d.ctl->xseq;
+  h.error = d.ctl->error;
+  const int last = d.n0 + d.nLoc - 1;
+  h.picks = d.ctl->error ? 0 : d.hDrawBase[last] + d.condDraws[last];
+  h.pad = 0;
+  for (int q = 0; q < d.G; ++q) hPickHdr(d, q)[d.rank] = h;
+}
+// after the wait (one thread): errors of the other shards; the test hook takes the serial path
+WTG_HD void hPickHeaders(const Dev& d) {
+  const XPick* h = hPickHdr(d, d.rank);
+  for (int q = 0; q < d.G; ++q) {
+    if (h[q].error && !d.ctl->error) setError(d, ERR_PEER_ERROR, q);
+    if (h[q].seq != d.ctl->xseq && !d.ctl->error) setError(d, ERR_INTERNAL, 730 + q);
+  }
+  if (d.forcePickSerial) d.ctl->hReject = 1;
+}
+// picks of the pass on the shards below shard q
+WTG_HD int hPicksBelow(const Dev& d, int q) {
+  int s = 0;
+  for (int p = 0; p < q; ++p) s += hPickHdr(d, d.rank)[p].picks;
+  return s;
+}
+// does pick t of the pass (counted over the shards up to this one) reject at its presumed position t?
+WTG_HD bool hPickRejects(const Dev& d, int t) {
+  const XPick* h = hPickHdr(d, d.rank);
+  int q = 0, base = 0;
+  while (q < d.rank && t >= base + h[q].picks) base += h[q++].picks;
+  int r;
+  return hNextInt(d, (u64)t, (int)hPickK(d, d.rank)[(size_t)q * (size_t)d.perShard + (size_t)(t - base)], r) > 1;
+}
+// one thread: the real positions of every pick of the pass, in shard and node order
+WTG_HD void hPickSerial(const Dev& d) {
+  u64 idx = 0;
+  int r;
+  for (int q = 0; q < d.rank; ++q) {
+    const unsigned char* ks = hPickK(d, d.rank) + (size_t)q * (size_t)d.perShard;
+    const int cnt = hPickHdr(d, d.rank)[q].picks;
+    for (int j = 0; j < cnt; ++j) idx += (u64)hNextInt(d, idx, (int)ks[j], r);
+  }
+  for (int n = d.n0; n < d.n0 + d.nLoc; ++n) idx += (u64)hCondPick(d, n, idx, true);
 }
 
 }  // namespace wtg

@@ -349,6 +349,7 @@ WTG_HD void xIngest(const Dev& d, C& c, int g) {
     const u64* from = xStagePtr(d, d.rank, src, (int)(uint32_t)pl);
     u64* dst = d.pool[l] + (size_t)slot * (size_t)nw;
     for (int w = c.lane(); w < nw; w += C::LANES) dst[w] = from[w];
+    if (d.proto == PROTO_HANDEL && c.lane() == 0) d.poolRef[l][slot] = 1;  // the reference the queue entry will hold
   }
   c.sync();
   if (c.lane() == 0) {
@@ -359,7 +360,7 @@ WTG_HD void xIngest(const Dev& d, C& c, int g) {
   c.sync();
 }
 WTG_HD bool xNeedsIngest(const Dev& d, int g) {
-  return d.proto == PROTO_GSF && d.newTarget[g] >= 0 && d.newEv[g].kind == EV_MSG && (d.newEv[g].meta & META_STAGED) != 0;
+  return (d.proto == PROTO_GSF || d.proto == PROTO_HANDEL) && d.newTarget[g] >= 0 && d.newEv[g].kind == EV_MSG && (d.newEv[g].meta & META_STAGED) != 0;
 }
 
 // ------------------------------------------------------------------------------------------
@@ -1976,8 +1977,12 @@ WTG_HD void emitDesc(const Dev& d, int di) {
         }
       }
     }
-    if (target < 0 && d.proto == PROTO_GSF && metaKind(ds.meta) == PK_POOL && !(ds.meta & META_STAGED))
+    // a dropped envelope takes its pooled payload with it: GSF's slab has no other owner, Handel's holds only the envelope's
+    // reference (hMakePayload).  A staged payload is never ingested (its staging area is reset every pass).
+    if (target < 0 && (d.proto == PROTO_GSF || d.proto == PROTO_HANDEL) && metaKind(ds.meta) == PK_POOL && !(ds.meta & META_STAGED))
       freeDirect(d, (int)metaLevel(ds.meta), (uint32_t)ds.pl);
+    else if (target >= 0 && shard && d.proto == PROTO_HANDEL && metaKind(ds.meta) == PK_POOL && ownerOf(d, (int)ev.to) != d.rank)
+      hStageAtEmit(d, ev);
   }
   if (d.farCap > 0) {
     if (target >= 0 && target - ctl.tick >= farHorizon(d)) {

@@ -10,7 +10,8 @@
 // arrivals with the global draw indices and stores each new envelope straight into the *destination* shard's
 // creation-indexed array over NVLink (peer stores; exchange 2), pooled payloads into a staging area of the destination.
 // The multisplit of every shard walks the creation-indexed array, so its buckets stay in the reference's order.
-// Synchronisation: per pass two flag words per peer (release / acquire at system scope), waited on by 1-block kernels.
+// Synchronisation: per pass two flag words per peer (a third for fast-forwarding protocols, another for Handel's pick
+// exchange; release / acquire at system scope), waited on by 1-block kernels.
 #pragma once
 #include "wtg_types.h"
 
@@ -80,7 +81,7 @@ WTG_HD CasperTabs casperTabsAt(char* base, int maxBlocks, int maxAtts) {
   t.cbIncluded = reinterpret_cast<unsigned long long*>(base + off);
   return t;
 }
-WTG_HD CasperTabs casperTabsOf(const Dev& d, int q) { return casperTabsAt(d.peer[q].casper, d.cMaxBlocks, d.cMaxAtts); }
+WTG_HD CasperTabs casperTabsOf(const Dev& d, int q) { return casperTabsAt(d.peer[q].proto, d.cMaxBlocks, d.cMaxAtts); }
 
 // ---- exchange 1: items -------------------------------------------------------------------------------------------
 // local conditional-task totals: the scan over [cond | items] holds them at the first item position

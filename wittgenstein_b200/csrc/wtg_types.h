@@ -162,20 +162,24 @@ struct XHdr {  // per pass and shard
 struct XBegin {  // fast-forwarding protocols (CasperIMD): what a shard knows about the next millisecond that holds an event
   int seq, next, after, error;
 };
+struct XPick {  // Handel: the picks (rd.nextInt(k) of checkSigs) a shard presumes for this pass, one draw each
+  int seq, picks, error, pad;
+};
 struct XAll {  // a sendAll of this pass: every shard builds the same sorted record from it (the record is replicated, not shipped)
   uint32_t from, meta;
   unsigned long long pl;
   int sendTime, g;
   unsigned long long draw;
 };
-constexpr uint32_t META_STAGED = 1u << 15;  // GSF: the pooled payload still sits in the staging area written by shard (meta >> 16) & 7
+constexpr uint32_t META_STAGED = 1u << 15;  // GSF / Handel: the pooled payload still sits in the staging area written by shard (meta >> 16) & 7
 constexpr int META_SRC_SHIFT = 16;
 struct MultiRec;
 struct Ev;
 struct Peer {  // exchange region of one shard as mapped into this process (own region included: peer[rank])
   XHdr* hdr;            // [G]            written by shard q at [q]
   XItem* items;         // [G][xItemCap]  written by shard q at [q][*]
-  int* flags;           // [3][G]         pass sequence number of the last completed publication (0: items, 1: envelopes, 2: next event)
+  int* flags;           // [4][G]         pass sequence number of the last completed publication (0: items, 1: envelopes, 2: next event,
+                        //                3: Handel picks)
   Ev* newEv;            // [newEvCap]     this tick's new envelopes, indexed by global creation index
   int* newTarget;       // [newEvCap]     arrival tick, -1 = nothing for this shard
   unsigned long long* stage;  // [2][G][stageCapWords] pooled payloads of envelopes addressed to this shard
@@ -185,7 +189,8 @@ struct Peer {  // exchange region of one shard as mapped into this process (own 
   XBegin* beg;          // [G]            written by shard q at [q] at the start of a pass (fast-forwarding protocols)
   XAll* all;            // [G][xAllCap]   sendAll descriptors of the pass, written by shard q at [q][*]
   int* allCnt;          // [G]
-  char* casper;         // CasperIMD: the block / attestation tables, replicated on every shard (writers store to all copies)
+  char* proto;          // protocol-specific: CasperIMD's block / attestation tables, replicated on every shard (writers store
+                        // to all copies); Handel's pick exchange (XPick [G], then k of every pick [G][perShard], wtg_handel.cuh)
 };
 
 struct CasperG {  // CasperIMD: block counter and the Byzantine producer's scalars (CasperIMD.java:511-518, 648-649)
@@ -459,6 +464,7 @@ struct Dev {
   unsigned long long* pool[MAX_LEVELS];  // slabs
   uint32_t* poolFree[MAX_LEVELS];        // free stacks
   int poolCap[MAX_LEVELS];
+  int forcePickSerial;  // test hook (Handel): always draw the checkSigs picks serially
 };
 
 }  // namespace wtg

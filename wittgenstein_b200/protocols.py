@@ -351,11 +351,13 @@ class HandelParameters:
 
 
 class Handel:
-    def __init__(self, params, _api=None, tunables=None):
+    def __init__(self, params, _api=None, tunables=None, shard=None, device=None):
+        """shard = (rank, world): this object is one node-id shard of a network spread over `world` engines (sharded.py);
+        its node-indexed read-backs cover its own ids."""
         self.params = params
         self._api = _api
         self._tunables = dict(tunables or {})
-        self._net = Network(_api)
+        self._net = Network(_api, device=device, shard=shard)
         self._net.set_network_latency(params.network_latency_name)  # Handel.java:214-215
         for k, v in self._tunables.items():
             self._net.set_tunable(k, v)
@@ -374,38 +376,44 @@ class Handel:
         self._net.api.check(self._net.api.handel_init(self._net.h, _p(arr, C.c_int)))
         self.levels = self._net.api.handel_levels(self._net.h)
         self.words = max(1, p.node_count // 64)
+        self.rows_local = self._net.local_count  # a shard reads back its own nodes
 
     def scalars(self):
-        n = self.params.node_count
+        n = self.rows_local
         out = np.zeros((9, n), np.int32)
         self._net.api.check(self._net.api.handel_node_scalars(self._net.h, _p(out, C.c_int)))
         keys = ["start_at", "pairing", "sigs_checked", "sig_queue_size", "msg_filtered", "window", "added_cycle", "total_sig_size", "queued"]
         return {k: out[i] for i, k in enumerate(keys)}
 
     def rows(self, which):
-        out = np.zeros((self.params.node_count, self.words), np.uint64)
+        out = np.zeros((self.rows_local, self.words), np.uint64)
         self._net.api.check(self._net.api.handel_rows(self._net.h, int(which), _p(out, C.c_ulonglong)))
         return out
 
     def level_scalars(self):
-        n, L = self.params.node_count, self.levels
+        n, L = self.rows_local, self.levels
         a = [np.zeros((n, L), np.int32) for _ in range(3)]
         self._net.api.check(self._net.api.handel_level_scalars(self._net.h, *[_p(v, C.c_int) for v in a]))
         return dict(pos=a[0], outgoing_finished=a[1], suicide_biz_after=a[2])
 
     def peers(self, node, level):
+        """emission list of `node` at `level`; on a sharded network only for the shard's own nodes"""
         out = np.zeros(max(1, self.params.node_count), np.int32)
         k = self._net.api.check(self._net.api.handel_peers(self._net.h, node, level, _p(out, C.c_int), self.params.node_count))
         return out[:k].copy()
 
     def ranks(self, node):
+        """receptionRanks of `node`; on a sharded network only for the shard's own nodes"""
         out = np.zeros(self.params.node_count, np.int32)
         self._net.api.check(self._net.api.handel_ranks(self._net.h, node, _p(out, C.c_int)))
         return out
 
     def continue_if(self):
-        """Handel.newContIf (:1044-1053)."""
+        """Handel.newContIf (:1044-1053); a shard answers for its own nodes."""
         c = self._net.counters()
         down = self._net.attrs()["down"]
+        if self._net.shard is not None:
+            n0, nl = self._net.shard_range()
+            down = down[n0:n0 + nl]
         sc = self.scalars()
         return bool((((c[4] == 0) | (sc["added_cycle"] > 0)) & (down == 0)).any())

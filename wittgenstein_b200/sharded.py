@@ -2,9 +2,10 @@
 
 Two ways to drive the same C ABI (include/wtg.h, `wtg_shard_*`):
 
-* `ShardedGSFSignature` — all shards in this process, one host thread per shard (the engines may sit on different GPUs
-  of the box, or share one): what a single-process caller such as the reference's JVM would do through JNI.
-* `DistributedGSFSignature` — one shard per process (torchrun: one rank per GPU); the 128-byte handles (CUDA IPC) of the
+* `ShardedGSFSignature`, `ShardedHandel`, `ShardedCasperIMD` — all shards in this process, one host thread per shard (the
+  engines may sit on different GPUs of the box, or share one): what a single-process caller such as the reference's JVM
+  would do through JNI.
+* `DistributedGSFSignature`, `DistributedHandel`, `DistributedCasperIMD` — one shard per process (torchrun: one rank per GPU); the 128-byte handles (CUDA IPC) of the
   exchange regions travel through `torch.distributed`, after that the data path is peer stores between the GPUs'
   kernels — no collective call per tick.
 
@@ -15,7 +16,7 @@ from concurrent.futures import ThreadPoolExecutor
 
 import numpy as np
 
-from .protocols import CasperIMD, GSFSignature
+from .protocols import CasperIMD, GSFSignature, Handel
 
 
 class _ShardedNetwork:
@@ -145,6 +146,61 @@ class ShardedGSFSignature:
             s.network().close()
 
 
+class ShardedHandel:
+    """Handel (BASELINE config #3) over `world` node-id shards driven from this process (one thread per shard).  Every shard
+    runs the whole host init; the level draws of checkSigs are ordered over the shards by the pick exchange, and pooled
+    payloads for another shard's nodes go through its staging area (DESIGN.md §8)."""
+
+    def __init__(self, params, world, devices=None, _api=None, tunables=None):
+        self.params = params
+        self.world = world
+        self.devices = list(devices) if devices is not None else [None] * world
+        self.shards = [Handel(params, _api, tunables, shard=(r, world), device=self.devices[r]) for r in range(world)]
+        self._pool = ThreadPoolExecutor(max_workers=world)
+        self._net = _ShardedNetwork(self)
+
+    def _each(self, fn):
+        return list(self._pool.map(fn, self.shards))
+
+    def network(self):
+        return self._net
+
+    def init(self):
+        self._each(lambda s: s.init())
+        handles = [s.network().shard_export() for s in self.shards]
+        self._each(lambda s: s.network().shard_link(handles))
+        self.levels = self.shards[0].levels
+        self.words = self.shards[0].words
+
+    def _owner(self, node):
+        return self.shards[node // (self.params.node_count // self.world)]
+
+    def scalars(self):
+        parts = self._each(lambda s: s.scalars())
+        return {k: np.concatenate([p[k] for p in parts]) for k in parts[0]}
+
+    def rows(self, which):
+        return np.concatenate(self._each(lambda s: s.rows(which)), axis=0)
+
+    def level_scalars(self):
+        parts = self._each(lambda s: s.level_scalars())
+        return {k: np.concatenate([p[k] for p in parts], axis=0) for k in parts[0]}
+
+    def peers(self, node, level):
+        return self._owner(node).peers(node, level)
+
+    def ranks(self, node):
+        return self._owner(node).ranks(node)
+
+    def continue_if(self):
+        return any(self._each(lambda s: s.continue_if()))
+
+    def close(self):
+        self._pool.shutdown(wait=True)
+        for s in self.shards:
+            s.network().close()
+
+
 class ShardedCasperIMD:
     """CasperIMD (BASELINE config #4) over `world` node-id shards driven from this process (one thread per shard): ids split
     into `world` contiguous ranges; the block and attestation tables are replicated (their creator stores into every copy),
@@ -257,3 +313,29 @@ class DistributedGSFSignature:
         t = torch.tensor([1 if self.local.continue_if() else 0], dtype=torch.int32, device=dev)
         self.dist.all_reduce(t, op=self.dist.ReduceOp.MAX)
         return bool(t.item())
+
+
+class DistributedHandel:
+    """This process's shard of a Handel network spread over the ranks of a torch.distributed group (one GPU each)."""
+
+    def __init__(self, params, dist, rank, world, device, tunables=None, _api=None):
+        self.params, self.dist, self.rank, self.world = params, dist, rank, world
+        self.local = Handel(params, _api, tunables, shard=(rank, world), device=device)
+
+    def network(self):
+        return self.local.network()
+
+    def init(self):
+        self.local.init()
+        mine = self.local.network().shard_export()
+        handles = [None] * self.world
+        self.dist.all_gather_object(handles, mine)
+        self.local.network().shard_link(handles)
+        self.dist.barrier()
+        self.levels, self.words = self.local.levels, self.local.words
+
+    def continue_if(self):
+        """Handel.newContIf over all shards: some live node of some shard has not finished (or still has extra cycles)"""
+        parts = [None] * self.world
+        self.dist.all_gather_object(parts, self.local.continue_if())
+        return any(parts)
