@@ -1,12 +1,15 @@
 // wittgenstein_b200 — CUDA backend (sm_90a, H100): the kernels of the tick pipeline and the C ABI.
 //
-// One simulated millisecond = one pass of this kernel sequence over SoA state resident in HBM:
-//   k_begin -> k_cond_mark / k_cond_nodes<scan> / k_cond_score / k_cond_nodes<select> (conditional tasks) ->
-//   k_dispatch_count -> pair scan A -> k_dispatch_scatter -> k_node_msgs (thread per node) / k_node_tasks (warp per
-//   node) -> pair scan B -> k_emit (seed / latency / arrival) -> multisplit (count, column scan, stable scatter
-//   into the time ring) -> k_free -> k_end
+// One simulated millisecond = one pass of these kernels over SoA state resident in HBM:
+//   k_begin -> { C: k_cond_mark / k_cond_nodes<scan> / k_cond_score / k_cond_nodes<select> (conditional tasks)
+//              | D: k_dispatch_count -> pair scan A -> k_dispatch_scatter }
+//   -> k_node_msgs (thread per node) / k_node_tasks (warp per node) -> pair scan B -> k_emit (seed / latency / arrival)
+//   -> { multisplit (count, column scan, stable scatter into the time ring) | k_free } -> k_end
+// The two chains inside braces run as two branches (two streams, fork / join edges in the tick graph) for unsharded
+// GSF and Handel engines in mode 1; otherwise, and in the profiled pass, one after the other in the order written.
 // All sizes are read from the device control block, so a whole runMs window is enqueued without
-// a host round trip.  See DESIGN.md §4 for why this reproduces the reference's sequential order.
+// a host round trip.  See DESIGN.md §4 for why this reproduces the reference's sequential order, and for what each
+// branch writes.
 #include <cuda_runtime.h>
 #include <unistd.h>
 
@@ -661,6 +664,8 @@ __global__ void k_gsf_shuffle(Dev d, int l, u64 s0, const int* liveRank, const u
 class CudaBackend : public Backend {
  public:
   cudaStream_t st = nullptr;
+  cudaStream_t side = nullptr;  // second branch of a pass (enqueueTick); joined back into st before the pass goes on
+  cudaEvent_t forkEv = nullptr, joinEv = nullptr;
   int devId = 0;  // every entry point binds it: callers may drive different networks from different host threads
   void bind() const { cudaSetDevice(devId); }
   int sms = 132;
@@ -703,6 +708,9 @@ class CudaBackend : public Backend {
     CUDA_OK(cudaGetDeviceProperties(&p, dev));
     sms = p.multiProcessorCount;
     CUDA_OK(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
+    CUDA_OK(cudaStreamCreateWithFlags(&side, cudaStreamNonBlocking));
+    CUDA_OK(cudaEventCreateWithFlags(&forkEv, cudaEventDisableTiming));
+    CUDA_OK(cudaEventCreateWithFlags(&joinEv, cudaEventDisableTiming));
     CUDA_OK(cudaDeviceGetAttribute(&smemOptin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
     CUDA_OK(cudaFuncSetAttribute(k_ms_count, cudaFuncAttributeMaxDynamicSharedMemorySize, smemOptin));
     CUDA_OK(cudaFuncSetAttribute(k_ms_scatter, cudaFuncAttributeMaxDynamicSharedMemorySize, smemOptin));
@@ -712,6 +720,9 @@ class CudaBackend : public Backend {
   ~CudaBackend() override {
     for (void* q : ipcOpened) cudaIpcCloseMemHandle(q);
     if (tickGraph) cudaGraphExecDestroy(tickGraph);
+    if (forkEv) cudaEventDestroy(forkEv);
+    if (joinEv) cudaEventDestroy(joinEv);
+    if (side) cudaStreamDestroy(side);
     if (st) cudaStreamDestroy(st);
   }
   void* alloc(size_t bytes) override {
@@ -848,9 +859,27 @@ class CudaBackend : public Backend {
     ++evUsed;
   }
 
+  // `side` starts at st's current position
+  void fork() {
+    CUDA_OK(cudaEventRecord(forkEv, st));
+    CUDA_OK(cudaStreamWaitEvent(side, forkEv, 0));
+  }
+  // st waits for everything queued on `side` so far
+  void join() {
+    CUDA_OK(cudaEventRecord(joinEv, side));
+    CUDA_OK(cudaStreamWaitEvent(st, joinEv, 0));
+  }
   void enqueueTick(const Dev& d, int mode) {
     const int wide = sms * 8;
     const size_t msSmem = (size_t)d.msWarps * d.ring * sizeof(int);
+    // Two branches per pass for the protocols with a conditional pass, in mode 1: the delivery dispatch (count, scan A,
+    // scatter) runs on `side` beside checkSigs, and k_free beside the multisplit.  Neither branch reads or writes what
+    // the other writes (DESIGN.md §4).  The profiled pass keeps the serial order on st, so that every kernel's
+    // event time is its own.  Under stream capture the fork and join become edges of the tick graph.
+    // Node-sharded engines keep one stream: their exchange kernels spin until every shard has signalled, and shards that
+    // share a GPU need a hardware queue each, or a spinning kernel can hold up another shard's publication behind it.
+    const bool branches = mode == 1 && !profiling && d.G == 1 && (d.proto == PROTO_GSF || d.proto == PROTO_HANDEL);
+    cudaStream_t sd = branches ? side : st;
     // mode 3: the host prepared the control block and the descriptors of sends it injects at the current time
     // (Engine::inject); only the emission half of the pipeline runs
     if (mode != 3) {
@@ -858,6 +887,7 @@ class CudaBackend : public Backend {
       k_begin<<<1, 32, 0, st>>>(d, mode);
       profEnd();
     }
+    if (branches) fork();
     if ((d.proto == PROTO_GSF || d.proto == PROTO_HANDEL) && mode != 3) {  // conditional tasks (checkSigs)
       // GSF's select keeps one bit per queue entry per warp in dynamic shared memory; Handel's scratch is static
       const size_t smem8 = d.proto == PROTO_GSF ? (size_t)8 * (size_t)(d.qcap / 32) * sizeof(uint32_t) : 0;
@@ -873,11 +903,14 @@ class CudaBackend : public Backend {
       profEnd();
       launches += 4;
       if (d.proto == PROTO_HANDEL) {  // draw scan and pick
+        // the draw scan's tile partials go to their own buffer: scan A may be running on `side` at the same time
+        Dev dd = d;
+        dd.scanPartial = d.drawScanPartial;
         profBegin(P_SCAN_PARTIAL);
-        k_scan_partial<<<wide, SCAN_THREADS, 0, st>>>(d, 2);
+        k_scan_partial<<<wide, SCAN_THREADS, 0, st>>>(dd, 2);
         profEnd();
         profBegin(P_SCAN_FINAL);
-        k_scan_final<<<wide, SCAN_THREADS, 0, st>>>(d, 2);
+        k_scan_final<<<wide, SCAN_THREADS, 0, st>>>(dd, 2);
         profEnd();
         if (d.G > 1) {  // node-sharded: the pick exchange puts the picks of the lower shards first
           profBegin(P_EXCHANGE);
@@ -900,17 +933,18 @@ class CudaBackend : public Backend {
     }
     if (mode != 2 && mode != 3) {  // dispatch and handlers
       profBegin(P_DISPATCH_COUNT);
-      k_dispatch_count<<<wide, 256, 0, st>>>(d);
+      k_dispatch_count<<<wide, 256, 0, sd>>>(d);
       profEnd();
       profBegin(P_SCAN_PARTIAL);
-      k_scan_partial<<<wide, SCAN_THREADS, 0, st>>>(d, 0);
+      k_scan_partial<<<wide, SCAN_THREADS, 0, sd>>>(d, 0);
       profEnd();
       profBegin(P_SCAN_FINAL);
-      k_scan_final<<<wide, SCAN_THREADS, 0, st>>>(d, 0);
+      k_scan_final<<<wide, SCAN_THREADS, 0, sd>>>(d, 0);
       profEnd();
       profBegin(P_DISPATCH_SCATTER);
-      k_dispatch_scatter<<<wide, 256, 0, st>>>(d);
+      k_dispatch_scatter<<<wide, 256, 0, sd>>>(d);
       profEnd();
+      if (branches) join();  // k_node_msgs appends deliveries to the queues checkSigs has just compacted
       profBegin(P_NODE);
       k_node_msgs<<<(d.nLoc + 255) / 256, 256, 0, st>>>(d);
       k_node_tasks<<<ARENA_STRIPES * 19, 256, 0, st>>>(d);
@@ -962,6 +996,7 @@ class CudaBackend : public Backend {
       }
       profEnd();
     }
+    if (branches) fork();  // every pool allocation of the pass (handlers, HiddenByzantine's pick) is behind us
     profBegin(P_MS_COUNT);
     k_ms_count<<<sms * 2, d.msWarps * 32, msSmem, st>>>(d);
     profEnd();
@@ -974,9 +1009,10 @@ class CudaBackend : public Backend {
     const bool pooled = d.proto == PROTO_GSF || d.proto == PROTO_HANDEL;  // only these protocols hold pooled payloads
     if (pooled) {
       profBegin(P_FREE);
-      k_free<<<ARENA_STRIPES * 2, 256, 0, st>>>(d);
+      k_free<<<ARENA_STRIPES * 2, 256, 0, sd>>>(d);
       profEnd();
     }
+    if (branches) join();
     profBegin(P_END);
     k_end<<<1, 1, 0, st>>>(d, mode);
     profEnd();

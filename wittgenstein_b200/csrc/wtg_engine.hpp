@@ -888,6 +888,7 @@ class Engine {
     d.hCand = dallocNodes<int>(32);
     d.hCandK = dallocNodes<int>();
     d.hDrawBase = dallocNodes<int>();
+    d.drawScanPartial = dalloc<int>(2 * 8192);
     d.hHidden = p.hiddenByzantine ? 1 : 0;
     d.forcePickSerial = forcePickSerial ? 1 : 0;
     d.hbNoPeers = dallocNodes<int>();

@@ -465,6 +465,7 @@ struct Dev {
   uint32_t* poolFree[MAX_LEVELS];        // free stacks
   int poolCap[MAX_LEVELS];
   int forcePickSerial;  // test hook (Handel): always draw the checkSigs picks serially
+  int* drawScanPartial;  // [2 * tiles] Handel: tile partials of the draw scan, apart from scanPartial (scan A runs beside it)
 };
 
 }  // namespace wtg
