@@ -73,8 +73,8 @@ int wtg_set_msg_discard_time(wtg_net* net, int ms);
 
 /* device capacities (no reference counterpart): "bcap", "qcap", "pool_slots_per_node", "desc_cap",
  * "rec_cap", "ring", "casper_votes", "casper_blocks", "stage_words" (node-sharded GSF / Handel: staging area for pooled payloads that
- * cross shards, 64-bit words per sending shard and pass parity); test hooks "force_shuffle_serial" (SanFermin family: the
- * serial shuffle path) and "force_pick_serial" (Handel: checkSigs' level draws walked serially, locally and across shards).  Exceeding a capacity makes wtg_run_ms fail loudly; it never drops events. */
+ * cross shards, 64-bit words per sending shard and pass parity); test hooks "force_shuffle_serial" (SanFermin family, Slush,
+ * Snowflake: the serial re-derivation of draw indices) and "force_pick_serial" (Handel: checkSigs' level draws walked serially, locally and across shards).  Exceeding a capacity makes wtg_run_ms fail loudly; it never drops events. */
 int wtg_set_tunable(wtg_net* net, const char* key, long long value);
 
 /* new PingPong(params).init() — protocols/PingPong.java:52-57, 82-87 */
@@ -96,6 +96,15 @@ int wtg_sanfermin_init(wtg_net* net);
  * params6 = { nodeCount, threshold, pairingTime, signatureSize, timeout, candidateCount } (SanFerminParameters :86-103).
  * Device engine: power-of-two nodeCount, candidateCount <= 63. */
 int wtg_cappos_init(wtg_net* net, const int* params6);
+
+/* new Slush(new SlushParameters(nodes, M, K, A, ...)).init() — protocols/Slush.java:36-74, and
+ * new Snowflake(new SnowflakeParameters(nodes, M, K, A, B, ...)).init() — protocols/Snowflake.java:38-88.
+ * AK = K * A is compared in double (onAnswer, Slush.java:161-176, Snowflake.java:170-188).  The sample of every query
+ * (randomRemotes, Slush.java:126-137, Snowflake.java:136-147) is drawn from network.rd at its exact position in the draw
+ * order.  1 <= K <= min(63, nodes - 1): with K >= nodes the reference never returns, with K = 0 it sends nothing.
+ * Not available on a node-sharded network. */
+int wtg_slush_init(wtg_net* net, int nodes, int M, int K, double A);
+int wtg_snowflake_init(wtg_net* net, int nodes, int M, int K, double A, int B);
 
 /* new Handel(params).init() — protocols/Handel.java:96-141, 957-1014.
  * params11 = { nodeCount, threshold, pairingTime, levelWaitTime, extraCycle, disseminationPeriodMs, fastPath, nodesDown,
@@ -195,6 +204,14 @@ int wtg_cappos_node_scalars(wtg_net* net, int* cpl, int* sigs, int* done, int* t
 /* java.util.Collections.shuffle(list, rnd) with rnd in 48-bit state `state` (JDK: for i = size; i > 1; i-- swap(i-1,
  * rnd.nextInt(i))); runs on the host the code the emit kernel uses; returns the number of values drawn from the stream */
 int wtg_java_shuffle(unsigned long long state, int n, int* inout);
+
+/* SlushNode / SnowflakeNode: myColor, myQueryNonce, round (Slush) or cnt (Snowflake), whether answerIP holds the Answer of
+ * the last query, and that Answer's colorsFound[1] / colorsFound[2] (0 when none is pending) — protocols/Slush.java:117-120,
+ * 217-231; protocols/Snowflake.java:127-130, 217-232 (Answer.round is never read by the reference and is not kept) */
+int wtg_avalanche_node_scalars(wtg_net* net, int* color, int* nonce, int* round_or_cnt, int* pending, int* found1, int* found2);
+/* pipeline passes whose rd draw indices were re-derived serially because a shuffle's nextInt rejected a value or a sample
+ * (randomRemotes) discarded an attempt (no reference counterpart; -1 on failure) */
+long long wtg_serial_passes(wtg_net* net);
 
 /* Handel read-backs on a node-sharded network: node_scalars, rows and level_scalars cover the shard's own ids (nLoc in place of
  * N); peers and ranks fail with "node belongs to another shard" for a node of another shard. */

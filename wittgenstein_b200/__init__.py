@@ -4,6 +4,6 @@ from ._lib import WtgError  # noqa: F401
 from .network import Network  # noqa: F401
 from .protocols import (CasperIMD, CasperParemeters, GSFSignature, GSFSignatureParameters, Handel, HandelParameters, PingPong,  # noqa: F401
                         PingPongParameters, SanFerminCappos, SanFerminCapposParameters, SanFerminSignature,
-                        SanFerminSignatureParameters)
+                        SanFerminSignatureParameters, Slush, SlushParameters, Snowflake, SnowflakeParameters)
 from .run_multiple import (DoneAtStatGetter, MsgReceivedStatGetter, ProgressPerTime, RunMultipleTimes, SimpleStats,  # noqa: F401
                            cont_until_done)

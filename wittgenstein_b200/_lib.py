@@ -52,6 +52,10 @@ class Api:
         "cappos_init": (C.c_int, [C.c_void_p, C.POINTER(C.c_int)]),
         "cappos_node_scalars": (C.c_int, [C.c_void_p] + [C.POINTER(C.c_int)] * 6 + [C.POINTER(C.c_longlong)]),
         "java_shuffle": (C.c_int, [C.c_ulonglong, C.c_int, C.POINTER(C.c_int)]),
+        "slush_init": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_double]),
+        "snowflake_init": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_double, C.c_int]),
+        "avalanche_node_scalars": (C.c_int, [C.c_void_p] + [C.POINTER(C.c_int)] * 6),
+        "serial_passes": (C.c_longlong, [C.c_void_p]),
         "handel_init": (C.c_int, [C.c_void_p, C.POINTER(C.c_int)]),
         "handel_node_scalars": (C.c_int, [C.c_void_p, C.POINTER(C.c_int)]),
         "handel_rows": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(C.c_ulonglong)]),

@@ -35,6 +35,44 @@ WTG_HD int javaShuffleAt(const u64* jumpA, const u64* jumpC, u64 s0, u64 idx, ui
   }
   return consumed;
 }
+// nextInt(bound) on the LCG state `st` (advanced in place); `consumed` counts the values drawn
+WTG_HD int javaNextIntStep(u64& st, int bound, int& consumed) {
+  for (;;) {
+    st = (st * 0x5DEECE66DULL + 0xBULL) & LCG_MASK;
+    ++consumed;
+    int32_t u = (int32_t)(uint32_t)(st >> 17);  // next(31)
+    if ((bound & (bound - 1)) == 0) return (int)(((long long)bound * (long long)u) >> 31);
+    int32_t r = u % bound;
+    if ((int32_t)((uint32_t)u - (uint32_t)r + (uint32_t)(bound - 1)) >= 0) return r;
+  }
+}
+// Slush / Snowflake randomRemotes() (Slush.java:126-137, Snowflake.java:136-147) from stream position `idx` after state `s0`:
+// one nextInt(n) per attempt until k distinct ids other than `self` are drawn, kept in draw order in `list`.  With
+// list == nullptr it only counts, without scratch memory: an id drawn before that is not the sender's was kept then (or
+// repeated a kept one), so ArrayList.contains is "drawn before", found by replaying the attempts.  Returns the number of
+// stream values consumed: k when no attempt hits the sender or repeats an id and no nextInt rejects.  The caller
+// guarantees 1 <= k <= min(n - 1, SHUFFLE_MAX - 1).
+WTG_HD int javaSampleAt(const u64* jumpA, const u64* jumpC, u64 s0, u64 idx, int self, int n, int k, uint32_t* list) {
+  const u64 st0 = lcgAdvance(jumpA, jumpC, s0, idx);
+  u64 st = st0;
+  int consumed = 0, cnt = 0;
+  while (cnt < k) {
+    const int before = consumed;
+    const int r = javaNextIntStep(st, n, consumed);
+    if (r == self) continue;
+    bool seen = false;  // ArrayList.contains
+    if (list) {
+      for (int i = 0; i < cnt; ++i) seen |= list[i] == (uint32_t)r;
+    } else {
+      u64 s2 = st0;
+      for (int c2 = 0; c2 < before && !seen;) seen = javaNextIntStep(s2, n, c2) == r;
+    }
+    if (seen) continue;
+    if (list) list[cnt] = (uint32_t)r;
+    ++cnt;
+  }
+  return consumed;
+}
 
 // SanFerminHelper.pickNextNodes(level, howMany) :123-157 without the shuffle (the emit step performs it): writes the new
 // list to `out` (at most howMany + 1 entries), returns its length.  usedNodes indices are the reference's raw ints: the
@@ -280,13 +318,15 @@ WTG_HD void cpHandle(const Dev& d, int n, uint32_t from, uint32_t type, u64 pl, 
 }
 
 // ------------------------------------------------------------------------------------------
-// draw bookkeeping of shuffled sends.  A descriptor's first draw sits at drawBase[item] + (draws of the event's earlier
-// descriptors); with shuffles a descriptor consumes nDest draws — unless nextInt's rejection loop fires somewhere in the
-// tick, which shifts every later draw: then shuffleSerial re-derives all draw indices of the tick in creation order.
+// draw bookkeeping of shuffled and sampled sends.  A descriptor's first draw sits at drawBase[item] + (draws of the event's
+// earlier descriptors); a shuffle consumes nDest draws with its seed, a sample nDest + 1 — unless nextInt's rejection loop
+// fires or an attempt of a sample is discarded somewhere in the tick, which shifts every later draw: then shuffleSerial
+// re-derives all draw indices of the tick in creation order.
 // ------------------------------------------------------------------------------------------
 WTG_HD int descDrawsNominal(const Desc& ds) {
   if (ds.dkind == DK_INSERT_AT) return 0;
   if (ds.dkind == DK_SEND_MULTI && (ds.aux & DESC_SHUFFLEK)) return (int)ds.nDest;
+  if (ds.dkind == DK_SEND_MULTI && (ds.aux & DESC_SAMPLEK)) return (int)ds.nDest + 1;
   if (ds.dkind == DK_SEND_MULTI && (ds.aux & DESC_SHUFFLE2)) return 2;
   return 1;
 }
@@ -309,11 +349,15 @@ WTG_HD void shuffleCheck(const Dev& d, int di) {
   if (ds.dkind == DK_SEND_MULTI && (ds.aux & DESC_SHUFFLEK)) {
     int consumed = javaShuffleAt(d.jumpA, d.jumpC, d.ctl->rng, descDrawOptimistic(d, di), nullptr, (int)ds.nDest);
     if (consumed != (int)ds.nDest - 1) d.ctl->shufReject = 1;
+  } else if (ds.dkind == DK_SEND_MULTI && (ds.aux & DESC_SAMPLEK)) {
+    int consumed = javaSampleAt(d.jumpA, d.jumpC, d.ctl->rng, descDrawOptimistic(d, di), (int)ds.from, d.N, (int)ds.nDest, nullptr);
+    if (consumed != (int)ds.nDest) d.ctl->shufReject = 1;
   }
 }
 WTG_HD void shuffleSerial(const Dev& d) {  // one thread
   Ctl& ctl = *d.ctl;
   if (!ctl.shufReject) return;
+  ctl.serialPasses += 1;
   u64 running = 0;
   for (int g = 0; g < ctl.totalSlots && g < d.newEvCap; ++g) {
     if (d.byGTick[g] != ctl.tick) continue;  // a conditional-task insert: no descriptor, no draw
@@ -323,6 +367,8 @@ WTG_HD void shuffleSerial(const Dev& d) {  // one thread
     if (ds.dkind == DK_INSERT_AT) continue;
     if (ds.dkind == DK_SEND_MULTI && (ds.aux & DESC_SHUFFLEK))
       running += (u64)javaShuffleAt(d.jumpA, d.jumpC, ctl.rng, running, nullptr, (int)ds.nDest);
+    else if (ds.dkind == DK_SEND_MULTI && (ds.aux & DESC_SAMPLEK))
+      running += (u64)javaSampleAt(d.jumpA, d.jumpC, ctl.rng, running, (int)ds.from, d.N, (int)ds.nDest, nullptr);
     else if (ds.dkind == DK_SEND_MULTI && (ds.aux & DESC_SHUFFLE2))
       running += 1;
     running += 1;  // the send's seed
@@ -330,14 +376,16 @@ WTG_HD void shuffleSerial(const Dev& d) {  // one thread
   ctl.totalDraws = (int)running;
 }
 
-// emit of a shuffled multi-send (up to SHUFFLE_MAX destinations): shuffle, seed, arrivals, stable sort, envelope
+// emit of a shuffled or sampled multi-send (up to SHUFFLE_MAX destinations): the list step (Collections.shuffle of the
+// handler's list, or randomRemotes filling it), seed, arrivals, stable sort, envelope
 WTG_HD void emitShuffled(const Dev& d, int di, int g, u64 drawIdx) {
   const Ctl& ctl = *d.ctl;
   const Desc& ds = d.desc[di];
   const int m = (int)ds.nDest;
   uint32_t* list = d.destScratch + ds.to;
   int* arr = reinterpret_cast<int*>(d.destScratch + ds.to + m);
-  int consumed = javaShuffleAt(d.jumpA, d.jumpC, ctl.rng, drawIdx, list, m);
+  int consumed = (ds.aux & DESC_SAMPLEK) ? javaSampleAt(d.jumpA, d.jumpC, ctl.rng, drawIdx, (int)ds.from, d.N, m, list)
+                                         : javaShuffleAt(d.jumpA, d.jumpC, ctl.rng, drawIdx, list, m);
   const int32_t seed = lcgNextIntAt(d, ctl.rng, drawIdx + (u64)consumed);
   const int from = (int)ds.from, sendTime = ctl.tick + 1;
   int cnt = 0;

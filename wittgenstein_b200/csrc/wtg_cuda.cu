@@ -208,7 +208,7 @@ __global__ void __launch_bounds__(256) k_node_msgs(Dev d) {
   u64 word = ~0ULL;
   if (n < d.n0 + d.nLoc && d.inboxFill[n] > 0) {
     CoopSerial cs;
-    if (d.proto == PROTO_SANFERMIN || d.proto == PROTO_CAPPOS)
+    if (d.proto == PROTO_SANFERMIN || d.proto == PROTO_CAPPOS || d.proto == PROTO_SLUSH || d.proto == PROTO_SNOWFLAKE)
       nodeProcess(d, cs, n, 0);
     else if (d.proto == PROTO_GSF || d.proto == PROTO_PINGPONG) {
       u64 w = 0;

@@ -1124,6 +1124,120 @@ class Engine {
     inited = true;
   }
 
+  // ---- Slush.init() / Snowflake.init()  (protocols/Slush.java:63-74, Snowflake.java:77-88): NODES_AV nodes on network.rd,
+  //      then node 0 takes colour 1 and node 1 colour 2, each calling sendQuery(1) — on the host, with the draws the emit
+  //      step would make (javaSampleAt, then the send's seed).  B < 0: Slush.  Ticks every millisecond like PingPong. ----
+  void slushInit(int N, int M, int K, double A, int B) {
+    requireNotInited();
+    requireUnsharded("this protocol");  // the samples are drawn in the emit step, in creation order over all nodes
+    if (N < 2) throw std::invalid_argument("NODES_AV must be at least 2");
+    if (K < 1 || K > N - 1 || K > SHUFFLE_MAX - 1)
+      throw std::invalid_argument("K must be in [1, min(63, NODES_AV - 1)]: with K >= NODES_AV randomRemotes never returns, with K = 0 "
+                                  "no query is sent");
+    checkLatencyBuilder();
+    hm.buildNodes(N);
+    const long long recs = tun.recCap ? tun.recCap : std::max<long long>(65536, 32LL * N);
+    recDestOverride = (int)std::min<long long>(0x7fffffffLL, recs * K + N + 1024);  // a record holds K destinations
+    allocCommon(N, B < 0 ? PROTO_SLUSH : PROTO_SNOWFLAKE);
+    d.sampleK = K;
+    d.sampleM = M;
+    d.sampleB = B;
+    d.sampleAK = (double)K * A;  // Slush: K * A, Snowflake: A * K (the same double)
+    std::vector<uint8_t> color((size_t)N, 0);
+    std::vector<int> nonce((size_t)N, 0);
+    std::vector<uint8_t> pend((size_t)N, 0);
+    d.avRound = dalloc<int>(N);
+    d.avFound = dalloc<uint8_t>((size_t)N * 2);
+    d.shufCap = d.newEvCap;
+    d.forceShufSerial = forceShufSerial ? 1 : 0;
+    d.byG = dalloc<int>(d.newEvCap);
+    {
+      std::vector<int> m1((size_t)d.newEvCap, -1);
+      d.byGTick = dupload(m1);
+    }
+    d.descDraw = dalloc<int>(d.descCap);
+    // the two initial queries: sendQuery(1) of node 0 (colour 1), then of node 1 (colour 2), both sent at time 0
+    Dev hd = hostView();
+    std::vector<long long> sent((size_t)N, 0);
+    std::vector<MultiRec> recs0;
+    std::vector<uint32_t> recDst;
+    std::vector<int> recArr;
+    std::vector<std::vector<Ev>> near((size_t)d.ring);
+    for (int n = 0; n < 2; ++n) {
+      color[(size_t)n] = (uint8_t)(n + 1);
+      nonce[(size_t)n] = 1;
+      pend[(size_t)n] = 1;
+      std::vector<uint32_t> list((size_t)K);
+      int used = javaSampleAt((const u64*)hostJumpA(), (const u64*)hostJumpC(), hm.rd.seed, 0, n, N, K, list.data());
+      hm.rd.seed = lcgAdvance((const u64*)hostJumpA(), (const u64*)hostJumpC(), hm.rd.seed, (u64)used);
+      int32_t seed = hm.rd.nextInt();
+      sent[(size_t)n] = K;  // msgSent++ / bytesSent += 1 per destination (Network.java:476-477)
+      struct Arr {
+        int arrival;
+        uint32_t dest;
+      };
+      std::vector<Arr> da;
+      for (uint32_t to : list) {
+        int nt = latency(hd, n, (int)to, pseudoRandom((int)to, seed));
+        if (nt < msgDiscardTime) da.push_back({1 + nt, to});
+      }
+      std::stable_sort(da.begin(), da.end(), [](const Arr& a, const Arr& b) { return a.arrival < b.arrival; });
+      if (da.empty()) continue;
+      Ev ev;
+      std::memset(&ev, 0, sizeof(ev));
+      ev.pad = 2;  // sent at time 0: sendTime 1 (+1)
+      ev.from = (uint32_t)n;
+      ev.meta = AV_QUERY;
+      ev.pl = avPl(1, n + 1);
+      ev.to = da[0].dest;
+      ev.kind = EV_MSG;
+      if (da.size() > 1) {
+        MultiRec rc;
+        std::memset(&rc, 0, sizeof(rc));
+        rc.pad = 2;
+        rc.from = (uint32_t)n;
+        rc.meta = AV_QUERY;
+        rc.pl = ev.pl;
+        rc.n = (uint32_t)da.size();
+        rc.off = (uint32_t)recDst.size();
+        ev.kind = EV_MULTI;
+        ev.aux = (uint32_t)recs0.size();
+        recs0.push_back(rc);
+        for (const Arr& a : da) {
+          recDst.push_back(a.dest);
+          recArr.push_back(a.arrival);
+        }
+      }
+      const int tgt = da[0].arrival;
+      if (da.back().arrival >= d.ring) throw std::runtime_error("latency exceeds the time ring");
+      near[(size_t)tgt].push_back(ev);
+    }
+    for (int t = 0; t < d.ring; ++t)
+      if (!near[(size_t)t].empty()) {
+        int c = (int)near[(size_t)t].size();
+        be->upload(d.buckets + (size_t)t * d.bcap, near[(size_t)t].data(), (size_t)c * sizeof(Ev));
+        be->upload(d.bucketCount + t, &c, sizeof(int));
+      }
+    if (!recs0.empty()) {
+      be->upload(d.rec, recs0.data(), recs0.size() * sizeof(MultiRec));
+      be->upload(d.recDest, recDst.data(), recDst.size() * sizeof(uint32_t));
+      be->upload(d.recArrival, recArr.data(), recArr.size() * sizeof(int));
+    }
+    be->upload(d.msgSent, sent.data(), sent.size() * sizeof(long long));
+    be->upload(d.bytesSent, sent.data(), sent.size() * sizeof(long long));
+    d.avColor = dupload(color);
+    d.avNonce = dupload(nonce);
+    d.avPend = dupload(pend);
+    Ctl c;
+    std::memset(&c, 0, sizeof(c));
+    c.callId = 1;
+    c.recTop = (int)recs0.size();
+    c.recDestTop = (int)recDst.size();
+    c.rng = hm.rd.seed;
+    writeCtl(c);
+    inited = true;
+  }
+
   // ---- CasperIMD: the constructor builds the observer (CasperIMD.java:81-88); init(byzantineNode) the producers and
   //      attesters with their periodic tasks (:478-508) ----
   CasperParams cp{};

@@ -1390,6 +1390,7 @@ WTG_HD int inboxEntry(u64 w) { return (int)(w & 0xFFFFFFFFULL); }
 #include "wtg_handel.cuh"
 #include "wtg_casper.cuh"
 #include "wtg_cappos.cuh"
+#include "wtg_avalanche.cuh"
 namespace wtg {
 
 // ------------------------------------------------------------------------------------------
@@ -1448,6 +1449,10 @@ WTG_HD void deliver(const Dev& d, C& c, int n, const Ev& ev, uint32_t from, uint
     draws = c.bcast(draws, 0);
   } else if (d.proto == PROTO_SANFERMIN) {
     if (c.lane() == 0) sfHandle(d, n, from, meta, pl, item, slots, draws);
+    slots = c.bcast(slots, 0);
+    draws = c.bcast(draws, 0);
+  } else if (d.proto == PROTO_SLUSH || d.proto == PROTO_SNOWFLAKE) {
+    if (c.lane() == 0) avHandle(d, n, from, meta, pl, item, slots, draws);
     slots = c.bcast(slots, 0);
     draws = c.bcast(draws, 0);
   } else if (d.proto == PROTO_PINGPONG) {
@@ -1883,9 +1888,9 @@ WTG_HD void emitDesc(const Dev& d, int di) {
   } else {
     u64 drawIdx = (u64)(d.drawBase[ds.item] + (int)ds.sub);
     if (shard) drawIdx += (u64)d.xoffD[ds.item - d.nLoc];
-    if (d.shufCap > 0) {  // protocols with k-element shuffles: draws per descriptor vary (wtg_cappos.cuh)
+    if (d.shufCap > 0) {  // protocols with k-element shuffles or samples: draws per descriptor vary (wtg_cappos.cuh)
       drawIdx = ctl.shufReject ? (u64)d.descDraw[di] : descDrawOptimistic(d, di);
-      if (ds.dkind == DK_SEND_MULTI && (ds.aux & DESC_SHUFFLEK)) {
+      if (ds.dkind == DK_SEND_MULTI && (ds.aux & (DESC_SHUFFLEK | DESC_SAMPLEK))) {
         emitShuffled(d, di, g, drawIdx);
         return;
       }

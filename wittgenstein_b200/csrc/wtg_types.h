@@ -30,7 +30,8 @@ constexpr int MAX_DIST = 1144;       // core/Node.java:17-18
 constexpr int MAX_SHARDS = 8;        // node-id shards of one simulation (one GPU each); power of two
 
 // protocols
-enum : int { PROTO_NONE = 0, PROTO_PINGPONG = 1, PROTO_GSF = 2, PROTO_SANFERMIN = 3, PROTO_HANDEL = 4, PROTO_CASPER = 5, PROTO_CAPPOS = 6 };
+enum : int { PROTO_NONE = 0, PROTO_PINGPONG = 1, PROTO_GSF = 2, PROTO_SANFERMIN = 3, PROTO_HANDEL = 4, PROTO_CASPER = 5, PROTO_CAPPOS = 6,
+             PROTO_SLUSH = 7, PROTO_SNOWFLAKE = 8 };
 
 // event kinds (Ev.kind)
 enum : uint32_t {
@@ -68,6 +69,11 @@ constexpr uint32_t DESC_SHUFFLEK = 2u;   // Desc.aux: Collections.shuffle of the
 constexpr uint32_t DESC_SENDTIME = 4u;   // Desc.aux: Desc.target holds the explicit send time (send(m, sendTime, from, ...), Network.java:369-447)
 constexpr int DESC_DELAY_SHIFT = 8;      // Desc.aux >> 8: delaysBetweenMessage of a multi-destination send (Network.java:420-467)
 constexpr uint32_t DESC_SHUFFLE2 = 1u;  // Desc.aux: Collections.shuffle of the 2 destinations before the send (one extra draw)
+constexpr uint32_t DESC_SAMPLEK = 8u;   // Desc.aux: the nDest destinations are drawn at emission (Slush / Snowflake randomRemotes:
+                                        // one nextInt(N) per attempt until nDest distinct ids other than the sender's; nDest draws
+                                        // when no attempt repeats an id or hits the sender)
+// Slush / Snowflake message types (Ev.meta); Ev.pl = query id | (colour << 32)
+enum : uint32_t { AV_QUERY = 1, AV_ANSWER = 2 };
 
 struct Ev {  // 32 bytes: one in-flight envelope / task
   uint32_t kind;
@@ -242,6 +248,7 @@ struct Ctl {  // device-resident control block (one per engine)
   int xNext, xAfter;             // global results of the begin exchange of this pass
   int poolMinFree[MAX_LEVELS];                 // low-water mark of free slots per level (sampled at tick end)
   int poolFreeCnt[MAX_LEVELS][POOL_STRIPES];   // free slots per (level, stripe)
+  long long serialPasses;        // passes whose draw indices shuffleSerial re-derived (shuffle rejections, sample collisions)
 };
 
 // striped statistics (node-id striping keeps hot-path counters off a single L2 address)
@@ -466,6 +473,14 @@ struct Dev {
   int poolCap[MAX_LEVELS];
   int forcePickSerial;  // test hook (Handel): always draw the checkSigs picks serially
   int* drawScanPartial;  // [2 * tiles] Handel: tile partials of the draw scan, apart from scanPartial (scan A runs beside it)
+  // ---- Slush / Snowflake (wtg_avalanche.cuh) ----
+  int sampleK, sampleM, sampleB;  // params.K, M, B (B < 0: Slush)
+  double sampleAK;                // params.AK = K * A, compared in double like the reference
+  uint8_t* avColor;   // [N] myColor (0 = uncoloured)
+  int* avNonce;       // [N] myQueryNonce
+  int* avRound;       // [N] Slush: round; Snowflake: cnt
+  uint8_t* avPend;    // [N] the Answer of query avNonce is open (at most one query per node is pending)
+  uint8_t* avFound;   // [N][2] its colorsFound[1], colorsFound[2]
 };
 
 }  // namespace wtg

@@ -321,6 +321,79 @@ class SanFerminCappos:
         return d
 
 
+class SlushParameters:
+    """Slush.SlushParameters (Slush.java:14-52); the defaults are the JSON constructor's (100, 4, 7, 4)."""
+
+    def __init__(self, nodes_av=100, m=4, k=7, a=4.0, node_builder_name=None, network_latency_name=None):
+        self.nodes_av = nodes_av
+        self.m = m
+        self.k = k
+        self.a = a
+        self.node_builder_name = node_builder_name
+        self.network_latency_name = network_latency_name
+
+
+class SnowflakeParameters:
+    """Snowflake.SnowflakeParameters (Snowflake.java:18-61); the defaults are the JSON constructor's (100, 4, 7, 4, 7)."""
+
+    def __init__(self, nodes_av=100, m=4, k=7, a=4.0, b=7, node_builder_name=None, network_latency_name=None):
+        self.nodes_av = nodes_av
+        self.m = m
+        self.k = k
+        self.a = a
+        self.b = b
+        self.node_builder_name = node_builder_name
+        self.network_latency_name = network_latency_name
+
+
+class _Avalanche:
+    """Slush / Snowflake (protocols/Slush.java, Snowflake.java): nodes are built by init(), which also sends the first two
+    queries (node 0 with colour 1, node 1 with colour 2)."""
+
+    def __init__(self, params, _api=None, tunables=None):
+        self.params = params
+        self._api = _api
+        self._tunables = dict(tunables or {})
+        self._net = Network(_api)
+        self._net.set_node_builder(params.node_builder_name)
+        self._net.set_network_latency(params.network_latency_name)
+        for k, v in self._tunables.items():
+            self._net.set_tunable(k, v)
+
+    def network(self):
+        return self._net
+
+    def copy(self):
+        return type(self)(self.params, self._api, self._tunables)
+
+    def scalars(self):
+        """per node: color, nonce, round (Slush) / cnt (Snowflake), pending, found1, found2 (colorsFound of the open query)"""
+        n = self.params.nodes_av
+        a = [np.zeros(n, np.int32) for _ in range(6)]
+        self._net.api.check(self._net.api.avalanche_node_scalars(self._net.h, *[_p(v, C.c_int) for v in a]))
+        return dict(zip(["color", "nonce", self._counter, "pending", "found1", "found2"], a))
+
+    def serial_passes(self):
+        """pipeline passes whose draw indices were re-derived serially (a query's sample discarded an attempt)"""
+        return self._net.api.check(self._net.api.serial_passes(self._net.h))
+
+
+class Slush(_Avalanche):
+    _counter = "round"
+
+    def init(self):
+        p = self.params
+        self._net.api.check(self._net.api.slush_init(self._net.h, int(p.nodes_av), int(p.m), int(p.k), float(p.a)))
+
+
+class Snowflake(_Avalanche):
+    _counter = "cnt"
+
+    def init(self):
+        p = self.params
+        self._net.api.check(self._net.api.snowflake_init(self._net.h, int(p.nodes_av), int(p.m), int(p.k), float(p.a), int(p.b)))
+
+
 class HandelParameters:
     """Handel.HandelParameters (Handel.java:22-142); window = WindowParameters() (16, 1, 128, ScoringExp(2, 4))."""
 
