@@ -213,6 +213,22 @@ int wtg_avalanche_node_scalars(wtg_net* net, int* color, int* nonce, int* round_
  * (randomRemotes) discarded an attempt (no reference counterpart; -1 on failure) */
 long long wtg_serial_passes(wtg_net* net);
 
+/* new P2PFlood(new P2PFloodParameters(nodeCount, deadNodeCount, delayBeforeResent, msgCount, msgToReceive, peersCount,
+ * delayBetweenSends, ...)).init() — protocols/P2PFlood.java:146-165 on core/P2PNetwork.java (setPeers, minimum = true) and
+ * core/messages/FloodMessage.java (msgToReceive is never read by the protocol).  Refused: negative arguments,
+ * peersCount >= nodeCount (the reference throws), msgCount above the live nodes (the reference never returns),
+ * delayBetweenSends >= 2^20, a peer graph with a degree above 256, record arenas beyond 2^31 entries, a node-sharded network. */
+int wtg_p2pflood_init(wtg_net* net, int nodeCount, int deadNodeCount, int delayBeforeResent, int msgCount, int peersCount,
+                      int delayBetweenSends);
+/* P2PNode.peers of `node` in the reference's order (link creation): its size; wtg_p2p_peers writes up to cap ids */
+int wtg_p2p_peer_count(wtg_net* net, int node);
+int wtg_p2p_peers(wtg_net* net, int node, int* out, int cap);
+/* P2PNetwork.avgPeers() (P2PNetwork.java:115-125) */
+int wtg_p2p_avg_peers(wtg_net* net);
+/* getMsgReceived(-1).size() of every node into count[N]; with bits != NULL also which originating messages (init's draw
+ * order) `node` holds, ceil(msgCount / 64) words (at least one).  Returns the number of words. */
+int wtg_p2pflood_received(wtg_net* net, int* count, int node, unsigned long long* bits);
+
 /* Handel read-backs on a node-sharded network: node_scalars, rows and level_scalars cover the shard's own ids (nLoc in place of
  * N); peers and ranks fail with "node belongs to another shard" for a node of another shard. */
 /* HNode fields — protocols/Handel.java:280-298: 9 int arrays of N: startAt, nodePairingTime, sigsChecked, sigQueueSize,

@@ -56,6 +56,11 @@ class Api:
         "snowflake_init": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_double, C.c_int]),
         "avalanche_node_scalars": (C.c_int, [C.c_void_p] + [C.POINTER(C.c_int)] * 6),
         "serial_passes": (C.c_longlong, [C.c_void_p]),
+        "p2pflood_init": (C.c_int, [C.c_void_p] + [C.c_int] * 6),
+        "p2p_peer_count": (C.c_int, [C.c_void_p, C.c_int]),
+        "p2p_peers": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(C.c_int), C.c_int]),
+        "p2p_avg_peers": (C.c_int, [C.c_void_p]),
+        "p2pflood_received": (C.c_int, [C.c_void_p, C.POINTER(C.c_int), C.c_int, C.POINTER(C.c_ulonglong)]),
         "handel_init": (C.c_int, [C.c_void_p, C.POINTER(C.c_int)]),
         "handel_node_scalars": (C.c_int, [C.c_void_p, C.POINTER(C.c_int)]),
         "handel_rows": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(C.c_ulonglong)]),

@@ -319,13 +319,14 @@ WTG_HD void cpHandle(const Dev& d, int n, uint32_t from, uint32_t type, u64 pl, 
 
 // ------------------------------------------------------------------------------------------
 // draw bookkeeping of shuffled and sampled sends.  A descriptor's first draw sits at drawBase[item] + (draws of the event's
-// earlier descriptors); a shuffle consumes nDest draws with its seed, a sample nDest + 1 — unless nextInt's rejection loop
-// fires or an attempt of a sample is discarded somewhere in the tick, which shifts every later draw: then shuffleSerial
-// re-derives all draw indices of the tick in creation order.
+// earlier descriptors); a shuffle consumes max(nDest, 1) draws with its seed (a send to an empty list still draws its seed,
+// Network.java:430), a sample nDest + 1 — unless nextInt's rejection loop fires or an attempt of a sample is discarded
+// somewhere in the tick, which shifts every later draw: then shuffleSerial re-derives all draw indices of the tick in
+// creation order.
 // ------------------------------------------------------------------------------------------
 WTG_HD int descDrawsNominal(const Desc& ds) {
   if (ds.dkind == DK_INSERT_AT) return 0;
-  if (ds.dkind == DK_SEND_MULTI && (ds.aux & DESC_SHUFFLEK)) return (int)ds.nDest;
+  if (ds.dkind == DK_SEND_MULTI && (ds.aux & DESC_SHUFFLEK)) return ds.nDest > 0 ? (int)ds.nDest : 1;
   if (ds.dkind == DK_SEND_MULTI && (ds.aux & DESC_SAMPLEK)) return (int)ds.nDest + 1;
   if (ds.dkind == DK_SEND_MULTI && (ds.aux & DESC_SHUFFLE2)) return 2;
   return 1;
@@ -348,7 +349,7 @@ WTG_HD void shuffleCheck(const Dev& d, int di) {
   if (d.forceShufSerial) d.ctl->shufReject = 1;
   if (ds.dkind == DK_SEND_MULTI && (ds.aux & DESC_SHUFFLEK)) {
     int consumed = javaShuffleAt(d.jumpA, d.jumpC, d.ctl->rng, descDrawOptimistic(d, di), nullptr, (int)ds.nDest);
-    if (consumed != (int)ds.nDest - 1) d.ctl->shufReject = 1;
+    if (consumed != (ds.nDest > 0 ? (int)ds.nDest - 1 : 0)) d.ctl->shufReject = 1;
   } else if (ds.dkind == DK_SEND_MULTI && (ds.aux & DESC_SAMPLEK)) {
     int consumed = javaSampleAt(d.jumpA, d.jumpC, d.ctl->rng, descDrawOptimistic(d, di), (int)ds.from, d.N, (int)ds.nDest, nullptr);
     if (consumed != (int)ds.nDest) d.ctl->shufReject = 1;

@@ -1001,6 +1001,7 @@ WTG_HD void tickBeginFfwd(const Dev& d, C& c) {
     ctl.hReject = 0;
     ctl.allCnt = 0;
     ctl.shufReject = 0;
+    ctl.peerCnt = 0;
     if (d.cg) d.cg->createdThisTick = 0;
     ctl.tieCnt = 0;
     if (d.G > 1) {

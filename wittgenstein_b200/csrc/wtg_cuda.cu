@@ -208,7 +208,8 @@ __global__ void __launch_bounds__(256) k_node_msgs(Dev d) {
   u64 word = ~0ULL;
   if (n < d.n0 + d.nLoc && d.inboxFill[n] > 0) {
     CoopSerial cs;
-    if (d.proto == PROTO_SANFERMIN || d.proto == PROTO_CAPPOS || d.proto == PROTO_SLUSH || d.proto == PROTO_SNOWFLAKE)
+    if (d.proto == PROTO_SANFERMIN || d.proto == PROTO_CAPPOS || d.proto == PROTO_SLUSH || d.proto == PROTO_SNOWFLAKE ||
+        d.proto == PROTO_P2PFLOOD)
       nodeProcess(d, cs, n, 0);
     else if (d.proto == PROTO_GSF || d.proto == PROTO_PINGPONG) {
       u64 w = 0;
@@ -486,6 +487,19 @@ __global__ void __launch_bounds__(128) k_emit_all(Dev d) {
   CoopWarp c;
   for (int j = gw; j < cnt; j += nw) emitAll(d, c, d.allList[j], d.allTmp + (size_t)gw * d.N, hist[warp]);
 }
+// P2PFlood forwards (DESC_PEERS descriptors): one warp each — the peer list and its shuffle in shared memory, arrivals, the
+// stably ranked record (wtg_p2p.cuh)
+__global__ void __launch_bounds__(128) k_emit_peers(Dev d) {
+  __shared__ uint32_t list[4][PEERS_MAX];
+  __shared__ int arr[4][PEERS_MAX];
+  if (d.ctl->error) return;
+  const int warp = threadIdx.x >> 5;
+  const int gw = blockIdx.x * 4 + warp, nw = gridDim.x * 4;
+  int cnt = d.ctl->peerCnt;
+  if (cnt > d.descCap) cnt = d.descCap;
+  CoopWarp c;
+  for (int j = gw; j < cnt; j += nw) emitPeers(d, c, d.peerList[j], list[warp], arr[warp]);
+}
 // node-sharded sendAll (CasperIMD): the descriptors are published to every shard before the envelope exchange ...
 __global__ void __launch_bounds__(128) k_x_all_publish(Dev d) {
   const int blk = blockIdx.x, nBlk = gridDim.x;
@@ -678,7 +692,7 @@ class CudaBackend : public Backend {
   cudaEvent_t tm0 = nullptr, tm1 = nullptr;
   // per-kernel profiling: one slot per timed group of kernels, reported under profNames[slot]
   enum ProfSlot { P_BEGIN, P_COND_SCAN, P_DISPATCH_COUNT, P_SCAN_PARTIAL, P_EXCHANGE, P_SCAN_FINAL, P_DISPATCH_SCATTER, P_NODE,
-                  P_EMIT, P_MS_COUNT, P_MS_SCAN, P_MS_SCATTER, P_FREE, P_END, P_COND_SCORE, P_COND_SELECT, NK };
+                  P_EMIT, P_MS_COUNT, P_MS_SCAN, P_MS_SCATTER, P_FREE, P_END, P_COND_SCORE, P_COND_SELECT, P_EMIT_PEERS, NK };
   bool profiling = false;
   std::vector<cudaEvent_t> evPool;
   std::vector<int> evKernel;  // kernel id of each event pair
@@ -687,7 +701,7 @@ class CudaBackend : public Backend {
   long long profCnt[NK] = {};
   const char* profNames[NK] = {"k_begin", "k_cond_scan", "k_dispatch_count", "k_scan_partial", "k_exchange", "k_scan_final",
                                "k_dispatch_scatter", "k_node", "k_emit", "k_ms_count", "k_ms_scan", "k_ms_scatter", "k_free",
-                               "k_end", "k_cond_score", "k_cond_select"};
+                               "k_end", "k_cond_score", "k_cond_select", "k_emit_peers"};
 
   explicit CudaBackend(int requested = -1) {
     int dev = 0;
@@ -985,6 +999,12 @@ class CudaBackend : public Backend {
       launches += 1;
     }
     profEnd();
+    if (d.proto == PROTO_P2PFLOOD) {
+      profBegin(P_EMIT_PEERS);
+      k_emit_peers<<<sms * 8, 128, 0, st>>>(d);
+      profEnd();
+      launches += 1;
+    }
     if (d.G > 1) {  // exchange 2: the envelopes were stored into their destination shards' arrays by k_emit
       profBegin(P_EXCHANGE);
       k_x_sync<<<1, 32, 0, st>>>(d, 1);

@@ -387,7 +387,8 @@ class Engine {
     }
     if (farEnabled) {
       d.ffwd = farTicking ? 0 : 1;
-      d.farCap = tun.farCap ? (int)tun.farCap : (farTicking ? (int)std::min<long long>(1LL << 26, std::max<long long>(64LL * N + 4096, farWanted)) : 2 * N + 1024);
+      d.farCap = tun.farCap ? (int)tun.farCap : (farTicking ? (int)std::min<long long>(1LL << 26, std::max<long long>(64LL * N + 4096, farWanted))
+                                                                  : (int)std::max<long long>(2LL * N + 1024, farWanted));
       d.far = dalloc<FarEv>(d.farCap);
       d.farSel = dalloc<int>(d.farCap);
     }
@@ -1234,6 +1235,168 @@ class Engine {
     c.recTop = (int)recs0.size();
     c.recDestTop = (int)recDst.size();
     c.rng = hm.rd.seed;
+    writeCtl(c);
+    inited = true;
+  }
+
+  // ---- P2PFlood.init()  (protocols/P2PFlood.java:146-165): nodeCount nodes on network.rd (the first deadNodeCount built
+  //      Byzantine and stopped), setPeers(), then rd.nextInt(nodeCount) until msgCount distinct live senders are drawn, each
+  //      calling sendPeers (P2PNetwork.java:127-132) at once — on the host, with the draws the emit step would make (the
+  //      shuffle of the sender's whole peer list, then the send's seed).  No conditional tasks: the calendar and
+  //      fast-forward run it, like CasperIMD. ----
+  std::vector<uint32_t> hPeerOff, hPeerIds;  // the peer graph (CSR), kept for the read-backs
+  void p2pFloodInit(int N, int dead, int resend, int msgCount, int peersCount, int between) {
+    requireNotInited();
+    requireUnsharded("this protocol");  // the shuffles are drawn in the emit step, in creation order over all nodes
+    if (N <= 0 || dead < 0 || resend < 0 || msgCount < 0 || peersCount < 0 || between < 0)
+      throw std::invalid_argument("P2PFlood parameters must not be negative (nodeCount > 0)");
+    if (between >= (1 << 20)) throw std::invalid_argument("delayBetweenSends must be below 2^20 (descriptor field)");
+    if (resend >= (1 << 30)) throw std::invalid_argument("delayBeforeResent must be below 2^30");
+    if (peersCount >= N)  // P2PNetwork.java:27-33
+      throw std::invalid_argument("Wrong configuration: #nodes=" + std::to_string(N) + ", connection target=" + std::to_string(peersCount));
+    const int live = N - std::min(dead, N);
+    if (msgCount > live)
+      throw std::invalid_argument("msgCount=" + std::to_string(msgCount) + " exceeds the " + std::to_string(live) +
+                                  " live nodes: the reference never finds that many senders");
+    checkLatencyBuilder();
+    hm.buildNodes(N);
+    for (int i = 0; i < std::min(dead, N); ++i) hm.nodes[(size_t)i].down = true;  // new P2PFloodNode(nb, true): stop()
+    buildPeerGraph(hm.rd, N, peersCount, hPeerOff, hPeerIds);
+    int maxDeg = 0;
+    for (int n = 0; n < N; ++n) maxDeg = std::max(maxDeg, (int)(hPeerOff[(size_t)n + 1] - hPeerOff[(size_t)n]));
+    if (maxDeg > PEERS_MAX)
+      throw std::invalid_argument("the peer graph has a node of degree " + std::to_string(maxDeg) + ": the emit warp shuffles at most " +
+                                  std::to_string(PEERS_MAX) + " peers");
+    // Every node forwards each message at most once (a stopped node started again included), and a forward keeps at most its
+    // degree of destinations: the record arenas never overflow, and the calendar holds every envelope in flight.
+    const long long recs = (long long)N * std::max(1, msgCount);
+    const long long dests = (long long)std::max(1, msgCount) * (long long)hPeerIds.size() + 1;
+    if (recs > 0x7fffffffLL || dests > 0x7fffffffLL)
+      throw std::invalid_argument("nodeCount x msgCount x degree does not fit the record arenas (2^31 entries)");
+    tun.recCap = recs;
+    recDestOverride = (int)dests;
+    farWanted = recs + 1024;
+    farEnabled = true;
+    allocCommon(N, PROTO_P2PFLOOD);
+    d.floodMsgs = msgCount;
+    d.floodWords = std::max(1, (msgCount + 63) / 64);
+    d.floodResend = resend;
+    d.floodBetween = between;
+    d.peerOff = dupload(hPeerOff);
+    d.peerIds = dupload(hPeerIds);
+    d.peerList = dalloc<int>(d.descCap);
+    d.shufCap = d.newEvCap;
+    d.forceShufSerial = forceShufSerial ? 1 : 0;
+    d.byG = dalloc<int>(d.newEvCap);
+    {
+      std::vector<int> m1((size_t)d.newEvCap, -1);
+      d.byGTick = dupload(m1);
+    }
+    d.descDraw = dalloc<int>(d.descCap);
+    // the senders and their sendPeers, in draw order
+    Dev hd = hostView();
+    std::vector<int> cnt((size_t)N, 0);
+    std::vector<unsigned long long> bits((size_t)N * d.floodWords, 0);
+    std::vector<long long> sent((size_t)N, 0), doneAt((size_t)N, 0);
+    std::vector<uint8_t> isSender((size_t)N, 0);
+    std::vector<MultiRec> recs0;
+    std::vector<uint32_t> recDst;
+    std::vector<int> recArr;
+    std::vector<std::vector<Ev>> near((size_t)d.ring);
+    std::vector<FarEv> far;
+    int farMin = 0x7fffffff;
+    const int sendTime = 1 + resend;  // time + 1 + msg.localDelay, at time 0
+    const int step = between > 0 ? between + 1 : 0;
+    for (int k = 0; k < msgCount;) {
+      const int from = hm.rd.nextInt(N);
+      if (hm.nodes[(size_t)from].down || isSender[(size_t)from]) continue;
+      isSender[(size_t)from] = 1;
+      const int msg = k++;
+      cnt[(size_t)from] = 1;  // msg.addToReceived(from)
+      bits[(size_t)from * d.floodWords + (size_t)(msg >> 6)] |= 1ULL << (msg & 63);
+      if (msgCount == 1) doneAt[(size_t)from] = 1;
+      std::vector<uint32_t> list(hPeerIds.begin() + hPeerOff[(size_t)from], hPeerIds.begin() + hPeerOff[(size_t)from + 1]);
+      for (int i = (int)list.size(); i > 1; --i) std::swap(list[(size_t)i - 1], list[(size_t)hm.rd.nextInt(i)]);  // Collections.shuffle
+      const int32_t seed = hm.rd.nextInt();
+      sent[(size_t)from] += (long long)list.size();
+      struct Arr {
+        int arrival;
+        uint32_t dest;
+      };
+      std::vector<Arr> da;
+      for (size_t i = 0; i < list.size(); ++i) {
+        const int to = (int)list[i];
+        if (hm.nodes[(size_t)from].down || hm.nodes[(size_t)to].down) continue;
+        const int nt = latency(hd, from, to, pseudoRandom(to, seed));
+        if (nt < msgDiscardTime) da.push_back({sendTime + (int)i * step + nt, (uint32_t)to});
+      }
+      std::stable_sort(da.begin(), da.end(), [](const Arr& a, const Arr& b) { return a.arrival < b.arrival; });
+      if (da.empty()) continue;
+      Ev ev;
+      std::memset(&ev, 0, sizeof(ev));
+      ev.pad = (uint32_t)sendTime + 1u;
+      ev.from = (uint32_t)from;
+      ev.meta = P2P_FLOOD;
+      ev.pl = (unsigned long long)msg;
+      ev.to = da[0].dest;
+      ev.kind = EV_MSG;
+      if (da.size() > 1) {
+        MultiRec rc;
+        std::memset(&rc, 0, sizeof(rc));
+        rc.pad = ev.pad;
+        rc.from = ev.from;
+        rc.meta = ev.meta;
+        rc.pl = ev.pl;
+        rc.n = (uint32_t)da.size();
+        rc.off = (uint32_t)recDst.size();
+        ev.kind = EV_MULTI;
+        ev.aux = (uint32_t)recs0.size();
+        recs0.push_back(rc);
+        for (const Arr& a : da) {
+          recDst.push_back(a.dest);
+          recArr.push_back(a.arrival);
+        }
+      }
+      const int tgt = da[0].arrival;
+      if (tgt < d.ring / 2) {
+        near[(size_t)tgt].push_back(ev);
+      } else {  // insertion order among calendar entries: creation order
+        FarEv f;
+        std::memset(&f, 0, sizeof(f));
+        f.ev = ev;
+        f.target = tgt;
+        f.key = (unsigned long long)msg;
+        far.push_back(f);
+        farMin = std::min(farMin, tgt);
+      }
+    }
+    for (int t = 0; t < d.ring; ++t)
+      if (!near[(size_t)t].empty()) {
+        const int c = (int)near[(size_t)t].size();
+        if (c > d.bcap) throw std::runtime_error("bucket capacity too small for the initial sends");
+        be->upload(d.buckets + (size_t)t * d.bcap, near[(size_t)t].data(), (size_t)c * sizeof(Ev));
+        be->upload(d.bucketCount + t, &c, sizeof(int));
+      }
+    if (!far.empty()) be->upload(d.far, far.data(), far.size() * sizeof(FarEv));
+    if (!recs0.empty()) {
+      be->upload(d.rec, recs0.data(), recs0.size() * sizeof(MultiRec));
+      be->upload(d.recDest, recDst.data(), recDst.size() * sizeof(uint32_t));
+      be->upload(d.recArrival, recArr.data(), recArr.size() * sizeof(int));
+    }
+    be->upload(d.msgSent, sent.data(), sent.size() * sizeof(long long));
+    be->upload(d.bytesSent, sent.data(), sent.size() * sizeof(long long));
+    be->upload(d.doneAt, doneAt.data(), doneAt.size() * sizeof(long long));
+    d.floodCnt = dupload(cnt);
+    d.floodBits = dupload(bits);
+    Ctl c;
+    std::memset(&c, 0, sizeof(c));
+    c.callId = 1;
+    c.recTop = (int)recs0.size();
+    c.recDestTop = (int)recDst.size();
+    c.rng = hm.rd.seed;
+    c.farCnt = (int)far.size();
+    c.farMin = farMin;
+    c.nextEvent = 0;  // unknown: the first window looks for itself
     writeCtl(c);
     inited = true;
   }

@@ -1391,6 +1391,7 @@ WTG_HD int inboxEntry(u64 w) { return (int)(w & 0xFFFFFFFFULL); }
 #include "wtg_casper.cuh"
 #include "wtg_cappos.cuh"
 #include "wtg_avalanche.cuh"
+#include "wtg_p2p.cuh"
 namespace wtg {
 
 // ------------------------------------------------------------------------------------------
@@ -1453,6 +1454,10 @@ WTG_HD void deliver(const Dev& d, C& c, int n, const Ev& ev, uint32_t from, uint
     draws = c.bcast(draws, 0);
   } else if (d.proto == PROTO_SLUSH || d.proto == PROTO_SNOWFLAKE) {
     if (c.lane() == 0) avHandle(d, n, from, meta, pl, item, slots, draws);
+    slots = c.bcast(slots, 0);
+    draws = c.bcast(draws, 0);
+  } else if (d.proto == PROTO_P2PFLOOD) {
+    if (c.lane() == 0) floodHandle(d, n, from, pl, item, slots, draws);
     slots = c.bcast(slots, 0);
     draws = c.bcast(draws, 0);
   } else if (d.proto == PROTO_PINGPONG) {
@@ -1890,6 +1895,16 @@ WTG_HD void emitDesc(const Dev& d, int di) {
     if (shard) drawIdx += (u64)d.xoffD[ds.item - d.nLoc];
     if (d.shufCap > 0) {  // protocols with k-element shuffles or samples: draws per descriptor vary (wtg_cappos.cuh)
       drawIdx = ctl.shufReject ? (u64)d.descDraw[di] : descDrawOptimistic(d, di);
+      if (ds.aux & DESC_PEERS) {  // built by emitPeers (wtg_p2p.cuh): on the device by k_emit_peers, a warp per forward
+#if !defined(__CUDA_ARCH__)
+        // the host build of these bodies has no separate warp pass: it runs the same body here with a one-lane group
+        CoopSerial cs;
+        uint32_t list[PEERS_MAX];
+        int arr[PEERS_MAX];
+        emitPeers(d, cs, di, list, arr);
+#endif
+        return;
+      }
       if (ds.dkind == DK_SEND_MULTI && (ds.aux & (DESC_SHUFFLEK | DESC_SAMPLEK))) {
         emitShuffled(d, di, g, drawIdx);
         return;
@@ -2060,6 +2075,7 @@ WTG_HD void tickBegin(const Dev& d, int mode) {
   c.hReject = 0;
   c.allCnt = 0;
   c.shufReject = 0;
+  c.peerCnt = 0;
   if (c.nEv > c.maxBucket) c.maxBucket = c.nEv;
   if (d.G > 1) {
     c.xseq += 1;

@@ -31,7 +31,7 @@ constexpr int MAX_SHARDS = 8;        // node-id shards of one simulation (one GP
 
 // protocols
 enum : int { PROTO_NONE = 0, PROTO_PINGPONG = 1, PROTO_GSF = 2, PROTO_SANFERMIN = 3, PROTO_HANDEL = 4, PROTO_CASPER = 5, PROTO_CAPPOS = 6,
-             PROTO_SLUSH = 7, PROTO_SNOWFLAKE = 8 };
+             PROTO_SLUSH = 7, PROTO_SNOWFLAKE = 8, PROTO_P2PFLOOD = 9 };
 
 // event kinds (Ev.kind)
 enum : uint32_t {
@@ -74,6 +74,11 @@ constexpr uint32_t DESC_SAMPLEK = 8u;   // Desc.aux: the nDest destinations are 
                                         // when no attempt repeats an id or hits the sender)
 // Slush / Snowflake message types (Ev.meta); Ev.pl = query id | (colour << 32)
 enum : uint32_t { AV_QUERY = 1, AV_ANSWER = 2 };
+constexpr uint32_t DESC_PEERS = 16u;  // Desc.aux: the destinations are the CSR peer row of Desc.from without node Desc.to (nDest of
+                                      // them), shuffled at emission by k_emit_peers (P2PFlood's FloodMessage forward)
+constexpr int PEERS_MAX = 256;        // longest peer list one emit warp shuffles (P2PFlood: maximum degree of the graph)
+// P2PFlood message type (Ev.meta); Ev.pl = index of the originating message (init's draw order)
+enum : uint32_t { P2P_FLOOD = 1 };
 
 struct Ev {  // 32 bytes: one in-flight envelope / task
   uint32_t kind;
@@ -249,6 +254,7 @@ struct Ctl {  // device-resident control block (one per engine)
   int poolMinFree[MAX_LEVELS];                 // low-water mark of free slots per level (sampled at tick end)
   int poolFreeCnt[MAX_LEVELS][POOL_STRIPES];   // free slots per (level, stripe)
   long long serialPasses;        // passes whose draw indices shuffleSerial re-derived (shuffle rejections, sample collisions)
+  int peerCnt;                   // DESC_PEERS descriptors of this pass (P2PFlood forwards, emitted by k_emit_peers)
 };
 
 // striped statistics (node-id striping keeps hot-path counters off a single L2 address)
@@ -481,6 +487,14 @@ struct Dev {
   int* avRound;       // [N] Slush: round; Snowflake: cnt
   uint8_t* avPend;    // [N] the Answer of query avNonce is open (at most one query per node is pending)
   uint8_t* avFound;   // [N][2] its colorsFound[1], colorsFound[2]
+  // ---- P2PFlood (wtg_p2p.cuh) ----
+  int floodMsgs, floodWords;  // params.msgCount, words of a node's bitmap (ceil(msgCount / 64))
+  int floodResend, floodBetween;  // FloodMessage.localDelay (delayBeforeResent), delayBetweenPeers (delayBetweenSends)
+  const uint32_t* peerOff;    // [N + 1] CSR: the peers of n are peerIds[peerOff[n] .. peerOff[n + 1]), in P2PNode.peers order
+  const uint32_t* peerIds;    // [sum of degrees]
+  int* floodCnt;              // [N] received(-1).size()
+  unsigned long long* floodBits;  // [N][floodWords] which of the originating messages the node has received
+  int* peerList;              // [descCap] DESC_PEERS descriptors of the pass (Ctl.peerCnt of them)
 };
 
 }  // namespace wtg

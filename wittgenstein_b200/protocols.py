@@ -394,6 +394,80 @@ class Snowflake(_Avalanche):
         self._net.api.check(self._net.api.snowflake_init(self._net.h, int(p.nodes_av), int(p.m), int(p.k), float(p.a), int(p.b)))
 
 
+class P2PFloodParameters:
+    """P2PFlood.P2PFloodParameters (P2PFlood.java:46-109); the defaults are the JSON constructor's (100, 10, 50, 1, 1, 10, 30).
+    msg_to_receive is kept for scenario code: the protocol itself never reads it."""
+
+    def __init__(self, node_count=100, dead_node_count=10, delay_before_resent=50, msg_count=1, msg_to_receive=1, peers_count=10,
+                 delay_between_sends=30, node_builder_name=None, network_latency_name=None):
+        self.node_count = node_count
+        self.dead_node_count = dead_node_count
+        self.delay_before_resent = delay_before_resent
+        self.msg_count = msg_count
+        self.msg_to_receive = msg_to_receive
+        self.peers_count = peers_count
+        self.delay_between_sends = delay_between_sends
+        self.node_builder_name = node_builder_name
+        self.network_latency_name = network_latency_name
+
+
+class P2PFlood:
+    """protocols/P2PFlood.java on a P2PNetwork (core/P2PNetwork.java, minimum = true): init() builds the nodes (the first
+    dead_node_count stopped), the peer graph, and sends msg_count messages from distinct live nodes to their peers.  Not
+    available on a node-sharded network."""
+
+    def __init__(self, params=None, _api=None, tunables=None):
+        self.params = params or P2PFloodParameters()
+        self._api = _api
+        self._tunables = dict(tunables or {})
+        self._net = Network(_api)
+        self._net.set_node_builder(self.params.node_builder_name)
+        self._net.set_network_latency(self.params.network_latency_name)
+        for k, v in self._tunables.items():
+            self._net.set_tunable(k, v)
+
+    def network(self):
+        return self._net
+
+    def copy(self):
+        return P2PFlood(self.params, self._api, self._tunables)
+
+    def init(self):
+        p = self.params
+        self._net.api.check(self._net.api.p2pflood_init(self._net.h, int(p.node_count), int(p.dead_node_count), int(p.delay_before_resent),
+                                                        int(p.msg_count), int(p.peers_count), int(p.delay_between_sends)))
+
+    def peers(self, i):
+        """P2PNode.peers of node i, in the reference's order (link creation)"""
+        api = self._net.api
+        k = api.check(api.p2p_peer_count(self._net.h, int(i)))
+        out = np.zeros(max(k, 1), np.int32)
+        api.check(api.p2p_peers(self._net.h, int(i), _p(out, C.c_int), k))
+        return out[:k]
+
+    def avg_peers(self):
+        """P2PNetwork.avgPeers()"""
+        return self._net.api.check(self._net.api.p2p_avg_peers(self._net.h))
+
+    def received_count(self):
+        """getMsgReceived(-1).size() of every node"""
+        out = np.zeros(self.params.node_count, np.int32)
+        self._net.api.check(self._net.api.p2pflood_received(self._net.h, _p(out, C.c_int), 0, None))
+        return out
+
+    def received(self, i):
+        """which originating messages (init's draw order) node i has received: a bool array of msg_count"""
+        cnt = np.zeros(self.params.node_count, np.int32)
+        words = max(1, (int(self.params.msg_count) + 63) // 64)
+        bits = np.zeros(words, np.uint64)
+        self._net.api.check(self._net.api.p2pflood_received(self._net.h, _p(cnt, C.c_int), int(i), _p(bits, C.c_ulonglong)))
+        return np.unpackbits(bits.view(np.uint8), bitorder="little")[:self.params.msg_count].astype(bool)
+
+    def serial_passes(self):
+        """pipeline passes whose draw indices were re-derived serially (a shuffle's nextInt rejected)"""
+        return self._net.api.check(self._net.api.serial_passes(self._net.h))
+
+
 class HandelParameters:
     """Handel.HandelParameters (Handel.java:22-142); window = WindowParameters() (16, 1, 128, ScoringExp(2, 4))."""
 
