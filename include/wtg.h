@@ -261,7 +261,8 @@ int wtg_gsf_peers(wtg_net* net, int node, int level, int* out, int cap);
 int wtg_stats(wtg_net* net, long long* out26);
 
 /* measurement hooks (no reference counterpart): a CUDA-event stopwatch on the engine's stream, and
- * per-kernel event timing of the tick pipeline (names[i] are static strings) */
+ * per-kernel event timing of the tick pipeline (names[i] are static strings; on = 2 reports the delivery dispatch's
+ * scan A under names of its own instead of adding it into scan B's) */
 int wtg_timer_start(wtg_net* net);
 double wtg_timer_stop_ms(wtg_net* net);
 int wtg_profile_enable(wtg_net* net, int on);

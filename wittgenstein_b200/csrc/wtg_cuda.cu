@@ -7,6 +7,8 @@
 //   -> { multisplit (count, column scan, stable scatter into the time ring) | k_free } -> k_end
 // The two chains inside braces run as two branches (two streams, fork / join edges in the tick graph) for unsharded
 // GSF and Handel engines in mode 1; otherwise, and in the profiled pass, one after the other in the order written.
+// Unsharded GSF in mode 1 goes one step further inside a runMs window: C of the next millisecond runs beside this
+// millisecond's emission (k_free -> k_cond_begin -> C | scan B -> k_emit -> multisplit), and the next pass starts at D.
 // All sizes are read from the device control block, so a whole runMs window is enqueued without
 // a host round trip.  See DESIGN.md §4 for why this reproduces the reference's sequential order, and for what each
 // branch writes.
@@ -33,20 +35,26 @@ constexpr int SCAN_THREADS = 256;
 constexpr int SCAN_ITEMS = 4;
 constexpr int SCAN_TILE = SCAN_THREADS * SCAN_ITEMS;
 
-__global__ void k_begin(Dev d, int mode) {  // one warp
+// condAhead: the pass's checkSigs has already run beside the previous pass's emission (k_begin), or the next pass's runs
+// beside this one's (k_end)
+__global__ void k_begin(Dev d, int mode, bool condAhead) {  // one warp
   if (threadIdx.x >= 32) return;
   if (d.ffwd && mode == 1) {
     CoopWarp c;
     tickBeginFfwd(d, c);
   } else if (d.farCap > 0 && !d.ffwd) {
     CoopWarp c;
-    tickBeginFar(d, c, mode);
+    tickBeginFar(d, c, mode, condAhead);
   } else if (threadIdx.x == 0) {
-    tickBegin(d, mode);
+    tickBegin(d, mode, condAhead);
   }
 }
-__global__ void k_end(Dev d, int mode) {
-  if (threadIdx.x == 0) tickEnd(d, mode);
+__global__ void k_end(Dev d, int mode, bool condAhead) {
+  if (threadIdx.x == 0) tickEnd(d, mode, condAhead);
+}
+// clock and counters of the next pass's checkSigs, which runs ahead (one thread: a few hundred bytes)
+__global__ void k_cond_begin(Dev d) {
+  if (threadIdx.x == 0) condBegin(d);
 }
 
 // ---- conditional tasks (checkSigs): scan -> score -> select ---------------------------------------
@@ -684,16 +692,22 @@ class CudaBackend : public Backend {
   void bind() const { cudaSetDevice(devId); }
   int sms = 132;
   int smemOptin = 0;
-  cudaGraphExec_t tickGraph = nullptr;
+  // one graph per pass shape (SHAPE_*): whether the pass runs its own checkSigs, and whether it runs the next pass's
+  enum { SHAPE_PLAIN, SHAPE_FIRST, SHAPE_LAST, SHAPE_MIDDLE, NSHAPES };
+  cudaGraphExec_t tickGraph[NSHAPES] = {};
+  long long shapeKernels[NSHAPES] = {};
   const void* graphFor = nullptr;
   bool useGraph = true;
   long long launches = 0;      // kernels enqueued (graph replays counted kernel by kernel)
-  long long graphKernels = 0;
   cudaEvent_t tm0 = nullptr, tm1 = nullptr;
   // per-kernel profiling: one slot per timed group of kernels, reported under profNames[slot]
+  // The dispatch's scan A has slots of its own; unless the caller asked for them apart (profileEnable(true, true)),
+  // profileRead adds them into scan B's k_scan_partial / k_scan_final.
   enum ProfSlot { P_BEGIN, P_COND_SCAN, P_DISPATCH_COUNT, P_SCAN_PARTIAL, P_EXCHANGE, P_SCAN_FINAL, P_DISPATCH_SCATTER, P_NODE,
-                  P_EMIT, P_MS_COUNT, P_MS_SCAN, P_MS_SCATTER, P_FREE, P_END, P_COND_SCORE, P_COND_SELECT, P_EMIT_PEERS, NK };
+                  P_EMIT, P_MS_COUNT, P_MS_SCAN, P_MS_SCATTER, P_FREE, P_END, P_COND_SCORE, P_COND_SELECT, P_EMIT_PEERS,
+                  P_SCAN_A_PARTIAL, P_SCAN_A_FINAL, NK };
   bool profiling = false;
+  bool profSplitScans = false;
   std::vector<cudaEvent_t> evPool;
   std::vector<int> evKernel;  // kernel id of each event pair
   size_t evUsed = 0;
@@ -701,7 +715,7 @@ class CudaBackend : public Backend {
   long long profCnt[NK] = {};
   const char* profNames[NK] = {"k_begin", "k_cond_scan", "k_dispatch_count", "k_scan_partial", "k_exchange", "k_scan_final",
                                "k_dispatch_scatter", "k_node", "k_emit", "k_ms_count", "k_ms_scan", "k_ms_scatter", "k_free",
-                               "k_end", "k_cond_score", "k_cond_select", "k_emit_peers"};
+                               "k_end", "k_cond_score", "k_cond_select", "k_emit_peers", "k_scan_a_partial", "k_scan_a_final"};
 
   explicit CudaBackend(int requested = -1) {
     int dev = 0;
@@ -733,7 +747,8 @@ class CudaBackend : public Backend {
   }
   ~CudaBackend() override {
     for (void* q : ipcOpened) cudaIpcCloseMemHandle(q);
-    if (tickGraph) cudaGraphExecDestroy(tickGraph);
+    for (cudaGraphExec_t g : tickGraph)
+      if (g) cudaGraphExecDestroy(g);
     if (forkEv) cudaEventDestroy(forkEv);
     if (joinEv) cudaEventDestroy(joinEv);
     if (side) cudaStreamDestroy(side);
@@ -820,9 +835,10 @@ class CudaBackend : public Backend {
     CUDA_OK(cudaEventElapsedTime(&ms, tm0, tm1));
     return (double)ms;
   }
-  void profileEnable(bool on) override {
+  void profileEnable(bool on, bool splitScans) override {
     sync();
     profiling = on;
+    profSplitScans = splitScans;
     if (on) {
       for (int i = 0; i < NK; ++i) {
         profMs[i] = 0;
@@ -832,11 +848,17 @@ class CudaBackend : public Backend {
   }
   int profileRead(double* ms, long long* cnt, const char** names, int cap) override {
     sync();
+    const int shown = profSplitScans ? NK : P_SCAN_A_PARTIAL;
     int k = 0;
-    for (int i = 0; i < NK && k < cap; ++i, ++k) {
+    for (int i = 0; i < shown && k < cap; ++i, ++k) {
       ms[k] = profMs[i];
       cnt[k] = profCnt[i];
       names[k] = profNames[i];
+      const int a = i == P_SCAN_PARTIAL ? P_SCAN_A_PARTIAL : i == P_SCAN_FINAL ? P_SCAN_A_FINAL : -1;
+      if (!profSplitScans && a >= 0) {
+        ms[k] += profMs[a];
+        cnt[k] += profCnt[a];
+      }
     }
     return k;
   }
@@ -883,7 +905,54 @@ class CudaBackend : public Backend {
     CUDA_OK(cudaEventRecord(joinEv, side));
     CUDA_OK(cudaStreamWaitEvent(st, joinEv, 0));
   }
-  void enqueueTick(const Dev& d, int mode) {
+  // checkSigs (C) on stream s: scan, score, select; Handel: draw scan and pick
+  void enqueueCond(const Dev& d, cudaStream_t s) {
+    const int wide = sms * 8;
+    // GSF's select keeps one bit per queue entry per warp in dynamic shared memory; Handel's scratch is static
+    const size_t smem8 = d.proto == PROTO_GSF ? (size_t)8 * (size_t)(d.qcap / 32) * sizeof(uint32_t) : 0;
+    profBegin(P_COND_SCAN);
+    k_cond_mark<<<(d.nLoc + 255) / 256, 256, 0, s>>>(d);
+    k_cond_nodes<0><<<ARENA_STRIPES * 19, 256, 0, s>>>(d);
+    profEnd();
+    profBegin(P_COND_SCORE);
+    k_cond_score<<<ARENA_STRIPES * 19, 256, 0, s>>>(d);
+    profEnd();
+    profBegin(P_COND_SELECT);
+    k_cond_nodes<1><<<ARENA_STRIPES * 19, 256, smem8, s>>>(d);
+    profEnd();
+    launches += 4;
+    if (d.proto == PROTO_HANDEL) {  // draw scan and pick
+      // the draw scan's tile partials go to their own buffer: scan A may be running on `side` at the same time
+      Dev dd = d;
+      dd.scanPartial = d.drawScanPartial;
+      profBegin(P_SCAN_PARTIAL);
+      k_scan_partial<<<wide, SCAN_THREADS, 0, s>>>(dd, 2);
+      profEnd();
+      profBegin(P_SCAN_FINAL);
+      k_scan_final<<<wide, SCAN_THREADS, 0, s>>>(dd, 2);
+      profEnd();
+      if (d.G > 1) {  // node-sharded: the pick exchange puts the picks of the lower shards first
+        profBegin(P_EXCHANGE);
+        k_hpick_publish<<<sms, 256, 0, s>>>(d);
+        k_x_sync<<<1, 32, 0, s>>>(d, 3);
+        profEnd();
+        profBegin(P_COND_SELECT);
+        k_hpick_xcheck<<<sms, 256, 0, s>>>(d);
+        k_hpick_xapply<<<sms, 256, 0, s>>>(d);
+        profEnd();
+        launches += 5;
+      } else {
+        profBegin(P_COND_SELECT);
+        k_hpick_check<<<sms, 256, 0, s>>>(d);
+        k_hpick_apply<<<sms, 256, 0, s>>>(d);
+        profEnd();
+        launches += 3;
+      }
+    }
+  }
+  // ownCond: the pass runs its own checkSigs (false: the previous pass ran it ahead).  nextCond: this pass runs the next
+  // pass's checkSigs beside its emission.  Both differ from true / false only for unsharded GSF in mode 1, unprofiled.
+  void enqueueTick(const Dev& d, int mode, bool ownCond = true, bool nextCond = false) {
     const int wide = sms * 8;
     const size_t msSmem = (size_t)d.msWarps * d.ring * sizeof(int);
     // Two branches per pass for the protocols with a conditional pass, in mode 1: the delivery dispatch (count, scan A,
@@ -893,72 +962,33 @@ class CudaBackend : public Backend {
     // Node-sharded engines keep one stream: their exchange kernels spin until every shard has signalled, and shards that
     // share a GPU need a hardware queue each, or a spinning kernel can hold up another shard's publication behind it.
     const bool branches = mode == 1 && !profiling && d.G == 1 && (d.proto == PROTO_GSF || d.proto == PROTO_HANDEL);
-    cudaStream_t sd = branches ? side : st;
+    // A pass whose checkSigs ran ahead has only the dispatch left before the handlers: it stays on st.  One that runs the
+    // next pass's checkSigs forks after the handlers: k_free, k_cond_begin and C on `side`, the emission on st.
+    const bool condBranch = branches && ownCond;
+    cudaStream_t sd = condBranch ? side : st;
     // mode 3: the host prepared the control block and the descriptors of sends it injects at the current time
     // (Engine::inject); only the emission half of the pipeline runs
     if (mode != 3) {
       profBegin(P_BEGIN);
-      k_begin<<<1, 32, 0, st>>>(d, mode);
+      k_begin<<<1, 32, 0, st>>>(d, mode, !ownCond);
       profEnd();
     }
-    if (branches) fork();
-    if ((d.proto == PROTO_GSF || d.proto == PROTO_HANDEL) && mode != 3) {  // conditional tasks (checkSigs)
-      // GSF's select keeps one bit per queue entry per warp in dynamic shared memory; Handel's scratch is static
-      const size_t smem8 = d.proto == PROTO_GSF ? (size_t)8 * (size_t)(d.qcap / 32) * sizeof(uint32_t) : 0;
-      profBegin(P_COND_SCAN);
-      k_cond_mark<<<(d.nLoc + 255) / 256, 256, 0, st>>>(d);
-      k_cond_nodes<0><<<ARENA_STRIPES * 19, 256, 0, st>>>(d);
-      profEnd();
-      profBegin(P_COND_SCORE);
-      k_cond_score<<<ARENA_STRIPES * 19, 256, 0, st>>>(d);
-      profEnd();
-      profBegin(P_COND_SELECT);
-      k_cond_nodes<1><<<ARENA_STRIPES * 19, 256, smem8, st>>>(d);
-      profEnd();
-      launches += 4;
-      if (d.proto == PROTO_HANDEL) {  // draw scan and pick
-        // the draw scan's tile partials go to their own buffer: scan A may be running on `side` at the same time
-        Dev dd = d;
-        dd.scanPartial = d.drawScanPartial;
-        profBegin(P_SCAN_PARTIAL);
-        k_scan_partial<<<wide, SCAN_THREADS, 0, st>>>(dd, 2);
-        profEnd();
-        profBegin(P_SCAN_FINAL);
-        k_scan_final<<<wide, SCAN_THREADS, 0, st>>>(dd, 2);
-        profEnd();
-        if (d.G > 1) {  // node-sharded: the pick exchange puts the picks of the lower shards first
-          profBegin(P_EXCHANGE);
-          k_hpick_publish<<<sms, 256, 0, st>>>(d);
-          k_x_sync<<<1, 32, 0, st>>>(d, 3);
-          profEnd();
-          profBegin(P_COND_SELECT);
-          k_hpick_xcheck<<<sms, 256, 0, st>>>(d);
-          k_hpick_xapply<<<sms, 256, 0, st>>>(d);
-          profEnd();
-          launches += 5;
-        } else {
-          profBegin(P_COND_SELECT);
-          k_hpick_check<<<sms, 256, 0, st>>>(d);
-          k_hpick_apply<<<sms, 256, 0, st>>>(d);
-          profEnd();
-          launches += 3;
-        }
-      }
-    }
+    if (condBranch) fork();
+    if ((d.proto == PROTO_GSF || d.proto == PROTO_HANDEL) && mode != 3 && ownCond) enqueueCond(d, st);  // conditional tasks
     if (mode != 2 && mode != 3) {  // dispatch and handlers
       profBegin(P_DISPATCH_COUNT);
       k_dispatch_count<<<wide, 256, 0, sd>>>(d);
       profEnd();
-      profBegin(P_SCAN_PARTIAL);
+      profBegin(P_SCAN_A_PARTIAL);
       k_scan_partial<<<wide, SCAN_THREADS, 0, sd>>>(d, 0);
       profEnd();
-      profBegin(P_SCAN_FINAL);
+      profBegin(P_SCAN_A_FINAL);
       k_scan_final<<<wide, SCAN_THREADS, 0, sd>>>(d, 0);
       profEnd();
       profBegin(P_DISPATCH_SCATTER);
       k_dispatch_scatter<<<wide, 256, 0, sd>>>(d);
       profEnd();
-      if (branches) join();  // k_node_msgs appends deliveries to the queues checkSigs has just compacted
+      if (condBranch) join();  // k_node_msgs appends deliveries to the queues checkSigs has just compacted
       profBegin(P_NODE);
       k_node_msgs<<<(d.nLoc + 255) / 256, 256, 0, st>>>(d);
       k_node_tasks<<<ARENA_STRIPES * 19, 256, 0, st>>>(d);
@@ -968,6 +998,14 @@ class CudaBackend : public Backend {
       }
       profEnd();
       launches += 6;
+    }
+    const bool pooled = d.proto == PROTO_GSF || d.proto == PROTO_HANDEL;  // only these protocols hold pooled payloads
+    if (nextCond) {  // every pool allocation and deferred free of the pass is behind us
+      fork();
+      k_free<<<ARENA_STRIPES * 2, 256, 0, side>>>(d);
+      k_cond_begin<<<1, 1, 0, side>>>(d);
+      enqueueCond(d, side);
+      launches += 2;
     }
     profBegin(P_SCAN_PARTIAL);
     k_scan_partial<<<wide, SCAN_THREADS, 0, st>>>(d, 1);
@@ -1016,7 +1054,7 @@ class CudaBackend : public Backend {
       }
       profEnd();
     }
-    if (branches) fork();  // every pool allocation of the pass (handlers, HiddenByzantine's pick) is behind us
+    if (branches && !nextCond) fork();  // every pool allocation of the pass (handlers, HiddenByzantine's pick) is behind us
     profBegin(P_MS_COUNT);
     k_ms_count<<<sms * 2, d.msWarps * 32, msSmem, st>>>(d);
     profEnd();
@@ -1026,17 +1064,16 @@ class CudaBackend : public Backend {
     profBegin(P_MS_SCATTER);
     k_ms_scatter<<<sms * 2, d.msWarps * 32, msSmem, st>>>(d);
     profEnd();
-    const bool pooled = d.proto == PROTO_GSF || d.proto == PROTO_HANDEL;  // only these protocols hold pooled payloads
-    if (pooled) {
+    if (pooled && !nextCond) {
       profBegin(P_FREE);
-      k_free<<<ARENA_STRIPES * 2, 256, 0, sd>>>(d);
+      k_free<<<ARENA_STRIPES * 2, 256, 0, branches ? side : st>>>(d);
       profEnd();
     }
     if (branches) join();
     profBegin(P_END);
-    k_end<<<1, 1, 0, st>>>(d, mode);
+    k_end<<<1, 1, 0, st>>>(d, mode, nextCond);
     profEnd();
-    launches += pooled ? 9 : 8;
+    launches += pooled && !nextCond ? 9 : 8;  // with nextCond, k_free was counted with k_cond_begin
   }
   // dynamic shared memory of the multisplit kernels: the attribute is per device and shared by every engine on it (several
   // engines may be driven from concurrent host threads), so it is set once, to the device's opt-in maximum
@@ -1050,29 +1087,45 @@ class CudaBackend : public Backend {
     enqueueTick(d, mode);
     CUDA_OK(cudaGetLastError());
   }
+  // A window of `count` mode-1 passes.  Unsharded GSF (cond_ahead on) runs the first pass with its own checkSigs and the
+  // next pass's, the middle ones with the next pass's only, the last with neither; a single pass keeps the plain shape.
+  // No checkSigs runs ahead across a call: between windows the host may change what it reads (stop / start nodes,
+  // partitions, injected sends), and the window's end-of-window pass (mode 2) runs its own.
   void ticks(const Dev& d, int count) override {
     bind();
     configure(d);
+    const bool ahead = d.condAhead != 0 && d.proto == PROTO_GSF && d.G == 1 && !profiling && count > 1;
+    auto shapeOf = [&](int i) { return !ahead ? SHAPE_PLAIN : i == 0 ? SHAPE_FIRST : i == count - 1 ? SHAPE_LAST : SHAPE_MIDDLE; };
+    auto enqueueShape = [&](int shape) { enqueueTick(d, 1, shape == SHAPE_PLAIN || shape == SHAPE_FIRST, shape == SHAPE_FIRST || shape == SHAPE_MIDDLE); };
     if (!useGraph || profiling || count < 4) {
-      for (int i = 0; i < count; ++i) enqueueTick(d, 1);
+      for (int i = 0; i < count; ++i) enqueueShape(shapeOf(i));
       CUDA_OK(cudaGetLastError());
       return;
     }
-    if (!tickGraph || graphFor != (const void*)d.ctl) {
-      if (tickGraph) cudaGraphExecDestroy(tickGraph);
-      cudaGraph_t g;
-      long long before = launches;
-      CUDA_OK(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
-      enqueueTick(d, 1);
-      CUDA_OK(cudaStreamEndCapture(st, &g));
-      graphKernels = launches - before;  // kernels per replay
-      launches = before;
-      CUDA_OK(cudaGraphInstantiate(&tickGraph, g, 0));
-      cudaGraphDestroy(g);
+    if (graphFor != (const void*)d.ctl) {
+      for (cudaGraphExec_t& g : tickGraph)
+        if (g) {
+          cudaGraphExecDestroy(g);
+          g = nullptr;
+        }
       graphFor = (const void*)d.ctl;
     }
-    for (int i = 0; i < count; ++i) CUDA_OK(cudaGraphLaunch(tickGraph, st));
-    launches += graphKernels * count;
+    for (int i = 0; i < count; ++i) {
+      const int shape = shapeOf(i);
+      if (!tickGraph[shape]) {
+        cudaGraph_t g;
+        long long before = launches;
+        CUDA_OK(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
+        enqueueShape(shape);
+        CUDA_OK(cudaStreamEndCapture(st, &g));
+        shapeKernels[shape] = launches - before;  // kernels per replay
+        launches = before;
+        CUDA_OK(cudaGraphInstantiate(&tickGraph[shape], g, 0));
+        cudaGraphDestroy(g);
+      }
+      CUDA_OK(cudaGraphLaunch(tickGraph[shape], st));
+      launches += shapeKernels[shape];
+    }
   }
   void gsfInitNodes(const Dev& d) override {
     bind();

@@ -69,7 +69,7 @@ struct Backend {
   // device-side timing (CUDA events on the engine's stream); no-ops on backends without a device
   virtual void timerStart() {}
   virtual double timerStopMs() { return 0.0; }
-  virtual void profileEnable(bool) {}
+  virtual void profileEnable(bool, bool) {}  // (on, report the dispatch's scan A apart from scan B)
   virtual int profileRead(double* ms, long long* launches, const char** names, int cap) { (void)ms; (void)launches; (void)names; (void)cap; return 0; }
   // node-sharded runs: one exchange region per shard that the other shards' kernels write into.  `allocShared` returns
   // zero-initialised memory that can be mapped by other processes; exportShared / importShared carry the 64-byte handle
@@ -348,13 +348,17 @@ class Engine {
     d.itemBase = dalloc<int>(d.bcap);
     d.evSlots = dalloc<int>(d.itemCap);
     d.evDraws = dalloc<int>(d.itemCap);
-    d.condFired = dallocNodes<int>();
+    // GSF: two halves, by the parity of checkSigs' tick (condHalf); the next pass's checkSigs may run beside this
+    // pass's emission, which reads the other half
+    d.condStride = proto == PROTO_GSF ? d.nLoc : 0;
+    d.condAhead = proto == PROTO_GSF && !sharded() ? condAhead : 0;
+    d.condFired = dalloc<int>((size_t)d.nLoc + d.condStride) - d.n0;
     d.condDraws = dallocNodes<int>();
     d.condDue = dallocNodes<int>();
     d.workCap = (int)std::max<long long>(1 << 16, 64LL * NL) / ARENA_STRIPES * ARENA_STRIPES;
     d.workList = dalloc<uint32_t>(d.workCap);
-    d.condEv = dallocNodes<Ev>();
-    d.condTarget = dallocNodes<int>();
+    d.condEv = dalloc<Ev>((size_t)d.nLoc + d.condStride) - d.n0;
+    d.condTarget = dalloc<int>((size_t)d.nLoc + d.condStride) - d.n0;
     d.slotBase = dalloc<int>((size_t)NL + d.itemCap);
     d.drawBase = dalloc<int>((size_t)NL + d.itemCap);
     d.scanPartial = dalloc<int>(2 * 8192);
@@ -397,6 +401,7 @@ class Engine {
   int destScratchOverride = 0;
   bool forceShufSerial = false;  // tunable force_shuffle_serial (test hook)
   bool forcePickSerial = false;  // tunable force_pick_serial (test hook, Handel)
+  int condAhead = 1;             // tunable cond_ahead (Dev::condAhead; 0 runs every pass's checkSigs in the pass)
   int ringExtra = 0;        // longest handler-chosen delay of a near envelope (e.g. blockConstructionTime)
   bool farEnabled = false;  // far-future calendar (+ fast-forward for protocols without conditional tasks)
   bool farTicking = false;  // calendar without fast-forward: the latency model, not the protocol, asked for it
@@ -1672,7 +1677,7 @@ class Engine {
     std::vector<int> ones((size_t)n, 1), zerosN((size_t)d.N, 0);
     be->upload(d.evSlots, ones.data(), ones.size() * sizeof(int));
     be->upload(d.evDraws, ones.data(), ones.size() * sizeof(int));
-    be->upload(d.condFired, zerosN.data(), zerosN.size() * sizeof(int));
+    be->upload(d.condFired + condHalf(d, time), zerosN.data(), zerosN.size() * sizeof(int));
     if (!scratch.empty()) be->upload(d.destScratch, scratch.data(), scratch.size() * sizeof(uint32_t));
     if (!allList.empty()) be->upload(d.allList, allList.data(), allList.size() * sizeof(int));
     {  // msgSent++ / bytesSent += size per destination (Network.java:476-477)

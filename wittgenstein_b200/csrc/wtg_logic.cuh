@@ -490,24 +490,28 @@ WTG_HD int gsfScorePool(const Dev& d, C& c, int n, uint32_t from, uint32_t meta,
 //   condMode 1: the clock has just ticked to `tick` inside a runMs window ending at `until`
 //   condMode 2: the reference's extra time++ past `until` at the end of the window
 // ------------------------------------------------------------------------------------------
+// Where the per-node outputs of the checkSigs pass of `tick` are: condFired / condEv / condTarget have two halves by tick
+// parity (GSF), so that the emission of one pass reads its own while the next pass's checkSigs writes the other half.
+WTG_HD size_t condHalf(const Dev& d, int tick) { return (size_t)(tick & 1) * (size_t)d.condStride; }
 // phase A, scalar part (one thread per node): is the conditional task examined now and is startIf true?
+// GSF's phases read the pass clock from condTick / condCall (see Ctl), not from tick / callId.
 WTG_HD bool gsfCondMark(const Dev& d, int n) {
   const Ctl& ctl = *d.ctl;
   bool dueNow = false;
   if (ctl.condMode != 0 && !d.ndown[n]) {
     int ms = d.minStart[n];
-    bool due = ctl.condMode == 1 ? (ms <= ctl.tick) : (ms <= ctl.until);
-    if (due && d.stamp[n] != ctl.callId) {
-      d.stamp[n] = ctl.callId;
+    bool due = ctl.condMode == 1 ? (ms <= ctl.condTick) : (ms <= ctl.until);
+    if (due && d.stamp[n] != ctl.condCall) {
+      d.stamp[n] = ctl.condCall;
       if (d.qLen[n] > 0) {  // startIf: !toVerify.isEmpty()
         dueNow = true;
-        d.minStart[n] = ctl.tick + d.pairing[n];
+        d.minStart[n] = ctl.condTick + d.pairing[n];
         statAdd(d, n, ST_CONDRUNS, 1ULL);
       }
     }
   }
   d.condDue[n] = dueNow ? 1 : 0;
-  if (!dueNow) d.condFired[n] = 0;
+  if (!dueNow) d.condFired[condHalf(d, ctl.condTick) + n] = 0;
   return dueNow;
 }
 
@@ -711,11 +715,11 @@ WTG_HD void gsfCondSelect(const Dev& d, C& c, int n, uint32_t* keepBits) {  // n
       ev.meta = best.meta;
       ev.pl = best.pl;
       ev.aux = 0;
-      ev.pad = (uint32_t)d.ctl->tick + 1u;  // Envelope.sendTime + 1 (EnvelopeInfo.sentAt for peekMessages; 0 = not recorded)
-      d.condEv[n] = ev;
-      d.condTarget[n] = ctl.tick + pairing;
+      ev.pad = (uint32_t)ctl.condTick + 1u;  // Envelope.sendTime + 1 (EnvelopeInfo.sentAt for peekMessages; 0 = not recorded)
+      d.condEv[condHalf(d, ctl.condTick) + n] = ev;
+      d.condTarget[condHalf(d, ctl.condTick) + n] = ctl.condTick + pairing;
     }
-    d.condFired[n] = found ? 1 : 0;
+    d.condFired[condHalf(d, ctl.condTick) + n] = found ? 1 : 0;
   }
 }
 
@@ -2026,27 +2030,30 @@ WTG_HD void emitDesc(const Dev& d, int di) {
 
 // conditional-task inserts come first in creation order (slot = scan over nodes)
 WTG_HD void emitCond(const Dev& d, int n) {
-  if (!d.condFired[n]) return;
+  const size_t h = condHalf(d, d.ctl->tick);
+  if (!d.condFired[h + n]) return;
   int g = d.slotBase[n - d.n0];
   if (d.G > 1) g += d.ctl->condXoffS;  // the lower shards' nodes come first
   if (g >= d.newEvCap) {
     setError(d, ERR_DESC_OVERFLOW, g);
     return;
   }
-  int target = d.condTarget[n];
+  int target = d.condTarget[h + n];
   if (target - d.ctl->tick >= d.ring) {
     setError(d, ERR_FAR_FUTURE, target);
     target = -1;
   }
   if (d.G > 1 && target < 0) return;
-  d.newEv[g] = d.condEv[n];
+  d.newEv[g] = d.condEv[h + n];
   d.newTarget[g] = target;
 }
 
 // ------------------------------------------------------------------------------------------
 // tick bookkeeping (single thread)
 // ------------------------------------------------------------------------------------------
-WTG_HD void tickBegin(const Dev& d, int mode) {
+// condAhead: this pass's checkSigs has already run, beside the previous pass's emission (k_cond_begin set its clock and
+// counters)
+WTG_HD void tickBegin(const Dev& d, int mode, bool condAhead = false) {
   Ctl& c = *d.ctl;
   if (mode == 1) {
     c.time += 1;  // nextMessage(): time++   (Network.java:541)
@@ -2065,9 +2072,15 @@ WTG_HD void tickBegin(const Dev& d, int mode) {
   for (int t = 0; t < ARENA_STRIPES; ++t) {
     c.descCnt[t] = 0;
     c.destCnt[t] = 0;
-    c.workCnt[t] = 0;
-    c.dueCnt[t] = 0;
+    if (!condAhead) {
+      c.workCnt[t] = 0;
+      c.dueCnt[t] = 0;
+    }
     c.taskCnt[t] = 0;
+  }
+  if (!condAhead) {
+    c.condTick = c.tick;
+    c.condCall = c.callId;
   }
   c.nItems = 0;
   c.totalSlots = 0;
@@ -2086,13 +2099,24 @@ WTG_HD void tickBegin(const Dev& d, int mode) {
 // tickBegin for protocols that keep the far-future calendar but tick every millisecond (conditional tasks): the calendar
 // entries that come within the horizon of this tick move to the head of their buckets first (one coop)
 template <class C>
-WTG_HD void tickBeginFar(const Dev& d, C& c, int mode) {
+WTG_HD void tickBeginFar(const Dev& d, C& c, int mode, bool condAhead = false) {
   if (mode != 2) farMigrate(d, c, mode == 1 ? d.ctl->time + 1 : d.ctl->time);
   c.sync();
-  if (c.lane() == 0) tickBegin(d, mode);
+  if (c.lane() == 0) tickBegin(d, mode, condAhead);
   c.sync();
 }
-WTG_HD void tickEnd(const Dev& d, int mode) {
+// GSF's pool low-water mark, sampled every 16 ticks after the pass's deferred frees
+WTG_HD void samplePoolMinFree(const Dev& d) {
+  Ctl& c = *d.ctl;
+  if (d.proto == PROTO_GSF && (c.tick & 15) == 0)
+    for (int l = INLINE_MAX_LEVEL + 1; l < d.L; ++l) {
+      int f = 0;
+      for (int t = 0; t < POOL_STRIPES; ++t) f += c.poolFreeCnt[l][t];
+      if (f < c.poolMinFree[l]) c.poolMinFree[l] = f;
+    }
+}
+// condAhead: the next pass's checkSigs ran beside this pass's emission; condBegin took the sample before its evictions
+WTG_HD void tickEnd(const Dev& d, int mode, bool condAhead = false) {
   Ctl& c = *d.ctl;
   c.rng = lcgAdvance(d.jumpA, d.jumpC, c.rng, (u64)c.totalDraws);
   c.statDraws += (unsigned long long)c.totalDraws;
@@ -2105,12 +2129,21 @@ WTG_HD void tickEnd(const Dev& d, int mode) {
   for (int t = 0; t < ARENA_STRIPES; ++t) c.freeCnt[t] = 0;
   if (d.proto == PROTO_CASPER && d.G > 1 && d.cg->createdThisTick > 1) setError(d, ERR_UNSUPPORTED, 4);  // unsharded: casperRenumber
   if (d.G > 1 && d.allCap > 0 && mode != 3) c.allSeq = (int)(((unsigned)c.allSeq + (unsigned)xAllTotal(d)) & 0x3fffffffu);  // record slots of the next pass
-  if (d.proto == PROTO_GSF && (c.tick & 15) == 0)
-    for (int l = INLINE_MAX_LEVEL + 1; l < d.L; ++l) {
-      int f = 0;
-      for (int t = 0; t < POOL_STRIPES; ++t) f += c.poolFreeCnt[l][t];
-      if (f < c.poolMinFree[l]) c.poolMinFree[l] = f;
-    }
+  if (!condAhead) samplePoolMinFree(d);
+}
+// Unsharded GSF, mode 1, after the handlers and the deferred frees of pass `tick` and before the checkSigs of pass tick + 1
+// runs ahead: that checkSigs's clock (the callId tickEnd will leave), condMode and counters, which the next tickBegin then
+// leaves alone; and this pass's pool sample, which the evictions of that checkSigs must not reach.
+WTG_HD void condBegin(const Dev& d) {
+  Ctl& c = *d.ctl;
+  samplePoolMinFree(d);
+  c.condTick = c.tick + 1;
+  c.condCall = c.callId + (c.nEv > 0 ? 1u : 0u);
+  c.condMode = 1;
+  for (int t = 0; t < ARENA_STRIPES; ++t) {
+    c.workCnt[t] = 0;
+    c.dueCnt[t] = 0;
+  }
 }
 // deferred frees -> pool free stacks (no allocation runs concurrently).  i indexes the striped list.
 WTG_HD void freeApply(const Dev& d, int i) {
@@ -2230,7 +2263,7 @@ WTG_HD Pair scanLoad(const Dev& d, int which, int j) {
     }
   } else {
     if (j < d.nLoc) {
-      p.a = d.condFired[d.n0 + j];
+      p.a = d.condFired[condHalf(d, d.ctl->tick) + d.n0 + j];
       p.b = d.condDraws[d.n0 + j];
     } else {
       p.a = d.evSlots[j - d.nLoc];

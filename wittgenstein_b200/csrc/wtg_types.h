@@ -255,6 +255,10 @@ struct Ctl {  // device-resident control block (one per engine)
   int poolFreeCnt[MAX_LEVELS][POOL_STRIPES];   // free slots per (level, stripe)
   long long serialPasses;        // passes whose draw indices shuffleSerial re-derived (shuffle rejections, sample collisions)
   int peerCnt;                   // DESC_PEERS descriptors of this pass (P2PFlood forwards, emitted by k_emit_peers)
+  // GSF's checkSigs reads its clock from these: tick and callId of the pass it belongs to.  tickBegin sets them to the
+  // pass's own; k_cond_begin sets them to the next pass's when that pass's checkSigs runs ahead (DESIGN.md §4)
+  int condTick;
+  uint32_t condCall;
 };
 
 // striped statistics (node-id striping keeps hot-path counters off a single L2 address)
@@ -348,10 +352,11 @@ struct Dev {
   int* evDraws;       // [itemCap] rd.nextInt() draws consumed by scan item
   int* condDue;       // [N] conditional task of node n is examined this tick and its queue is not empty
   uint32_t* workList; // [workCap] global queue-entry index (n*qcap+i) of stale pooled entries, striped
-  int* condFired;     // [N]
+  int* condFired;     // [N], GSF: [2][N]: the half of checkSigs' tick parity (condHalf)
   int* condDraws;     // [N] rd draws consumed by the node's conditional task this tick (Handel: nextInt(k))
-  Ev* condEv;         // [N] task created by the conditional task of node n
-  int* condTarget;    // [N]
+  Ev* condEv;         // [N] task created by the conditional task of node n; GSF: [2][N] like condFired
+  int* condTarget;    // [N]; GSF: [2][N] like condFired
+  int condStride;     // elements between the two halves of condFired / condEv / condTarget (GSF: nLoc; others: 0, one copy)
   int* slotBase;      // [N + itemCap]
   int* drawBase;      // [N + itemCap]
   int* scanPartial;   // [2 * tiles]
@@ -478,6 +483,8 @@ struct Dev {
   uint32_t* poolFree[MAX_LEVELS];        // free stacks
   int poolCap[MAX_LEVELS];
   int forcePickSerial;  // test hook (Handel): always draw the checkSigs picks serially
+  int condAhead;        // unsharded GSF: 0 = every pass runs its own checkSigs; 1 = the next pass's runs beside the emission tail
+                        // (host build: before the tail; 2: after it)
   int* drawScanPartial;  // [2 * tiles] Handel: tile partials of the draw scan, apart from scanPartial (scan A runs beside it)
   // ---- Slush / Snowflake (wtg_avalanche.cuh) ----
   int sampleK, sampleM, sampleB;  // params.K, M, B (B < 0: Slush)

@@ -191,8 +191,10 @@ class Network:
     def timer_stop_ms(self):
         return float(self.api.timer_stop_ms(self.h))
 
-    def profile_enable(self, on=True):
-        self.api.check(self.api.profile_enable(self.h, 1 if on else 0))
+    def profile_enable(self, on=True, split_scans=False):
+        """split_scans: profile_read reports the delivery dispatch's scan A as k_scan_a_partial / k_scan_a_final; by default
+        it is added into k_scan_partial / k_scan_final, which scan B (and Handel's draw scan) report"""
+        self.api.check(self.api.profile_enable(self.h, (2 if split_scans else 1) if on else 0))
 
     def profile_read(self):
         cap = 64
