@@ -746,16 +746,21 @@ WTG_HD void emitAllCore(const Dev& d, C& c, uint32_t fromU, uint32_t meta, u64 p
   }
   bool keep = true;  // this engine holds the bucket entry of the first group
   if (cnt > 1) {
-    int ri = 0;
+    int ri = 0, samePass = 0;
     if (shard)
       ri = (int)((unsigned)seq % (unsigned)d.recSlots);
-    else if (c.lane() == 0)
-      ri = (int)((unsigned)WTG_ATOMIC_ADD(&d.ctl->recTop, 1) % (unsigned)d.recSlots);
+    else if (c.lane() == 0) {
+      const unsigned raw = (unsigned)WTG_ATOMIC_ADD(&d.ctl->recTop, 1);
+      ri = (int)(raw % (unsigned)d.recSlots);
+      // an earlier sendAll of this pass took the slot: the warps emit in parallel, so its record may not be written yet
+      samePass = raw - (unsigned)ctl.allRecBase >= (unsigned)d.recSlots;
+    }
     ri = c.bcast(ri, 0);
+    samePass = c.bcast(samePass, 0);
     MultiRec old = d.rec[ri];
     // the slot still holds a live envelope?  (replicated records: the cursor lives in the bucket entries, so a slot is
     // free once its last arrival has been processed)
-    const bool live = shard ? (old.n > 0 && d.recArrival[old.off + old.n - 1] > ctl.tick) : (old.cur < old.n);
+    const bool live = samePass || (shard ? (old.n > 0 && d.recArrival[old.off + old.n - 1] > ctl.tick) : (old.cur < old.n));
     if (live) {
       setError(d, ERR_REC_OVERFLOW, ri);
       cnt = 0;
@@ -908,7 +913,8 @@ WTG_HD void farMigrate(const Dev& d, C& c, int t) {
   Ctl& ctl = *d.ctl;
   const int limit = t + farHorizon(d) - 1;
   if (ctl.farMin > limit) return;
-  const int cnt = ctl.farCnt;
+  // farAppend keeps counting past farCap once the calendar has overflowed (the error is final): read only what it holds
+  const int cnt = ctl.farCnt < d.farCap ? ctl.farCnt : d.farCap;
   int nsel = 0;
   for (int i0 = 0; i0 < cnt; i0 += C::LANES) {
     int i = i0 + c.lane();
@@ -1000,6 +1006,7 @@ WTG_HD void tickBeginFfwd(const Dev& d, C& c) {
     ctl.totalDraws = 0;
     ctl.hReject = 0;
     ctl.allCnt = 0;
+    ctl.allRecBase = ctl.recTop;
     ctl.shufReject = 0;
     ctl.peerCnt = 0;
     if (d.cg) d.cg->createdThisTick = 0;

@@ -1779,9 +1779,11 @@ class Engine {
     long long s = 0;
     for (int b = 0; b < d.ring; ++b)
       if (bc[(size_t)b] > 0) s += countBucket(b, bc[(size_t)b]);
-    if (d.farCap > 0) s += readCtl().farCnt;
+    if (d.farCap > 0) s += farHeld();
     return (int)s;
   }
+  // entries of the far-future calendar: farCnt keeps counting past farCap once the calendar has overflowed
+  int farHeld() { return std::min(readCtl().farCnt, d.farCap); }
   int msgsSizeAt(int t) {
     requireInited();
     if (t < time) return 0;
@@ -1790,9 +1792,8 @@ class Engine {
     if (t < time + d.ring) be->download(&v, d.bucketCount + (t & ringMask), sizeof(int));
     if (v > 0) v = countBucket(t & ringMask, v);
     if (d.farCap > 0) {
-      Ctl c = readCtl();
-      std::vector<FarEv> far((size_t)c.farCnt);
-      if (c.farCnt) be->download(far.data(), d.far, far.size() * sizeof(FarEv));
+      std::vector<FarEv> far((size_t)farHeld());
+      if (!far.empty()) be->download(far.data(), d.far, far.size() * sizeof(FarEv));
       for (const FarEv& f : far)
         if (f.target == t) ++v;
     }
@@ -1880,9 +1881,8 @@ class Engine {
       for (const Ev& e : evs) addOne(e, arrival);
     }
     if (d.farCap > 0) {
-      Ctl c = readCtl();
-      std::vector<FarEv> far((size_t)c.farCnt);
-      if (c.farCnt) be->download(far.data(), d.far, far.size() * sizeof(FarEv));
+      std::vector<FarEv> far((size_t)farHeld());
+      if (!far.empty()) be->download(far.data(), d.far, far.size() * sizeof(FarEv));
       for (const FarEv& f : far) addOne(f.ev, f.target);
     }
     std::stable_sort(out.begin(), out.end(), [](const PeekRow& a, const PeekRow& b) {

@@ -2087,6 +2087,7 @@ WTG_HD void tickBegin(const Dev& d, int mode, bool condAhead = false) {
   c.totalDraws = 0;
   c.hReject = 0;
   c.allCnt = 0;
+  c.allRecBase = c.recTop;
   c.shufReject = 0;
   c.peerCnt = 0;
   if (c.nEv > c.maxBucket) c.maxBucket = c.nEv;

@@ -259,6 +259,7 @@ struct Ctl {  // device-resident control block (one per engine)
   // pass's own; k_cond_begin sets them to the next pass's when that pass's checkSigs runs ahead (DESIGN.md §4)
   int condTick;
   uint32_t condCall;
+  int allRecBase;  // recTop when this pass's sendAlls began taking record slots (CasperIMD's recycled slots, one engine)
 };
 
 // striped statistics (node-id striping keeps hot-path counters off a single L2 address)
